@@ -858,19 +858,20 @@ static int32_t query_device_impl(filo_ctx* ctx, const filo_table* t, int32_t fn,
   cudaEvent_t& e0 = evp.e0; cudaEvent_t& e1 = evp.e1;
 
   // ---- kernel selection.  v2 (TMA-staged, blocked reductions) needs its whole per-warp working set in shared memory;
-  //      v1 (generic, global-memory record reads, optional global scratch) takes everything else.  FILO_KERNEL=v1 forces v1.
+  //      v1 (generic, global-memory record reads, optional global scratch) takes everything else.  The v4 kernels and the tile
+  //      kernel run in front of v2 where they apply.  FILO_KERNEL=v1 forces v1, v2 forces v2, v3 keeps the SUM class on the tile
+  //      kernel (the other classes on v2).
   const uint32_t acc_bytes = fused ? align_up((uint32_t)q.T * 12u, 128) : 0;
-  const bool delta_fn = (fn == FILO_FN_DELTA);
   const bool need_corr2 = need_corr && t->any_drop;
   uint32_t scratch2 = align_up((uint32_t)t->max_chunks * (uint32_t)CHUNK_DESC_BYTES, 16) +
                       ((uint32_t)t->max_rows + (uint32_t)t->max_chunks * 8u) * 8u * (1u + (t->any_nonconst_ts ? 1u : 0u) + (need_corr2 ? 1u : 0u));
   scratch2 = align_up(scratch2 + 16, 128);
-  (void)delta_fn;
   const uint32_t rec_cap = align_up(t->max_rec_bytes + 16, 128);
   const size_t per_warp2 = v2_smem_per_warp(rec_cap, scratch2, acc_bytes);
-  const char* force = std::getenv("FILO_KERNEL");
-  const bool want_v1 = force && std::string(force) == "v1";
-  const bool use_v2 = !want_v1 && t->max_rec_bytes > 0 && per_warp2 * FAST_WARPS + 1024 <= std::min<size_t>(ctx->max_smem_optin, 227 * 1024);
+  const char* force_env = std::getenv("FILO_KERNEL");
+  const std::string force = force_env ? force_env : "";
+  const size_t smem_cap = std::min<size_t>(ctx->max_smem_optin, 227 * 1024);
+  const bool use_v2 = force != "v1" && t->max_rec_bytes > 0 && per_warp2 * FAST_WARPS + 1024 <= smem_cap;
   const int64_t work = fused ? t->n_items : t->n_series;
   int64_t launches = 0;
   uint8_t* gscratch = nullptr;
@@ -892,82 +893,62 @@ static int32_t query_device_impl(filo_ctx* ctx, const filo_table* t, int32_t fn,
     if (!use_smem) CUDA_TRY(ctx, tmp.alloc((void**)&gscratch, (size_t)L.grid * SCAN_WARPS * (scratch + acc_bytes)));
     L.gscratch = gscratch; L.scratch_bytes = scratch; L.use_smem = use_smem;
   }
-  // v3 tile kernel (scan_tile.cuh): SUM-class functions over regular series; irregular series are appended to a list that the
-  // v2 kernel processes right after, into the same output buffer.  FILO_KERNEL=v2 disables the tile kernel.
-  const bool want_v2 = force && std::string(force) == "v2";
   const int fn_cls = fn_class_of(fn, q.cumulative, q.long_values);
-  // zero rows around a chunk let clamped windows run without bounds checks: a window spans at most window/step + 1 rows
-  // at either end; when that does not leave room for two CTAs per SM the tile kernel falls back to checked loads
-  TileSmem TL;
-  {
-    const bool ctr = fn_cls == CLASS_COUNTER;
-    const uint64_t wrows = (uint64_t)(q.window / q.step) + 1;
-    const uint32_t full_pad = ctr ? 0u : (uint32_t)std::min<uint64_t>(2 * wrows, 1u << 20) + 16;
-    static const bool warp_decode = [] { const char* e = std::getenv("FILO_TILE_WARPDEC"); return e && e[0] == '1'; }();   // experimental
-    const bool wdec = warp_decode;
-    TL = tile_layout(t->max_rec_bytes, (uint32_t)t->max_rows, (uint32_t)q.T, full_pad, ctr, wdec);
-    if (((size_t)TL.total + 1024) * 2 > (size_t)228 * 1024) TL = tile_layout(t->max_rec_bytes, (uint32_t)t->max_rows, (uint32_t)q.T, ctr ? 0u : 16u, ctr, wdec);
-    // junction blocks made C2 slower (the blocks share a
-    // strided item list with the regular blocks, so every warp runs both paths): off unless FILO_TILE_JUNCTION=1
-    static const bool junction = [] { const char* e = std::getenv("FILO_TILE_JUNCTION"); return e && e[0] == '1'; }();
-    if (!junction) TL.opts &= ~TILE_OPT_JUNCTION;
+  const uint64_t wrows = (uint64_t)(q.window / q.step) + 1;
+  // v3 tile kernel (scan_tile.cuh): SUM-class functions over regular series; irregular series are appended to a list that the
+  // v2 kernel processes right after, into the same output buffer.  Zero rows around a chunk let clamped windows run without
+  // bounds checks: a window spans at most window/step + 1 rows at either end; when that does not leave room for two CTAs per SM
+  // the tile kernel falls back to checked loads.
+  TileSmem TL{};
+  bool use_tile = false;
+  if (use_v2 && force != "v2" && fn_cls == CLASS_SUM && t->n_series > 0) {
+    TL = tile_layout(t->max_rec_bytes, (uint32_t)t->max_rows, (uint32_t)q.T, (uint32_t)std::min<uint64_t>(2 * wrows, 1u << 20) + 16);
+    if (((size_t)TL.total + 1024) * 2 > (size_t)228 * 1024) TL = tile_layout(t->max_rec_bytes, (uint32_t)t->max_rows, (uint32_t)q.T, 16);
+    use_tile = (size_t)TL.total + 1024 <= smem_cap;
   }
-  const bool use_tile = use_v2 && !want_v2 && (fn_cls == CLASS_SUM || fn_cls == CLASS_COUNTER) && t->n_series > 0 &&
-                        (size_t)TL.total + 1024 <= std::min<size_t>(ctx->max_smem_optin, 227 * 1024);
-  // v4 warp-pipeline kernel (scan_wp.cuh): SUM-class functions without a fused aggregate; what it declines goes to the v2 kernel like the
-  // tile kernel's declines.  FILO_KERNEL=v3 keeps the tile kernel.
-  WpSmem WL;
+  // v4 SUM kernel (scan_wp.cuh): per-series rows, in front of the tile kernel; what it declines goes to the v2 kernel
+  WpSmem WL{};
   bool use_wp = false;
-  {
-    const uint64_t wrows = (uint64_t)(q.window / q.step) + 1;
-    const bool want_v3 = force && std::string(force) == "v3";
-    if (use_tile && !want_v3 && fn_cls == CLASS_SUM && wrows <= 4096 && t->max_chunks > 0) {
-      const size_t cap = std::min<size_t>(ctx->max_smem_optin, 227 * 1024);
-      static const int warps_env = [] { const char* e = std::getenv("FILO_WP_WARPS"); return e ? atoi(e) : 0; }();
-      static const bool no_alias = [] { const char* e = std::getenv("FILO_WP_ALIAS"); return e && e[0] == '0'; }();
-      // O in V's place (more warps per SM) when every series is summed in one pass of <= 64 blocks
-      const bool alias = !no_alias && wp_max_items((uint32_t)t->max_chunks, (uint32_t)q.T, (uint32_t)wrows) <= 64;
-      WL = wp_layout(t->max_rec_bytes, (uint32_t)t->max_rows, (uint32_t)t->max_chunks, (uint32_t)q.T, (uint32_t)wrows, alias);
-      size_t w = cap / WL.per_warp; const size_t wmax = alias ? WP_MAX_WARPS_ALIAS : WP_MAX_WARPS; if (w > wmax) w = wmax;
-      if (warps_env > 0 && (size_t)warps_env < w) w = (size_t)warps_env;
-      WL.warps = (uint32_t)w;
-      use_wp = w >= 4;
-    }
+  if (use_tile && force != "v3" && wrows <= 4096 && t->max_chunks > 0) {
+    // O in V's place (more warps per SM) when every series is summed in one pass of <= 64 blocks
+    const bool alias = wp_max_items((uint32_t)t->max_chunks, (uint32_t)q.T, (uint32_t)wrows) <= 64;
+    WL = wp_layout(t->max_rec_bytes, (uint32_t)t->max_rows, (uint32_t)t->max_chunks, (uint32_t)q.T, (uint32_t)wrows, alias);
+    WL.warps = (uint32_t)std::min<size_t>(smem_cap / WL.per_warp, alias ? WP_MAX_WARPS_ALIAS : WP_MAX_WARPS);
+    use_wp = WL.warps >= 4;
   }
-  // v4 counter-class kernel (scan_wp_ctr.cuh), per-series rows or fused partial rows
-  auto wp_ctr_plan = [&](bool agg_mode, WpCtrSmem& W) -> bool {
-    const bool want_v3 = force && std::string(force) == "v3";
-    if (!use_tile || want_v3 || fn_cls != CLASS_COUNTER || t->max_chunks <= 0) return false;
-    W = wp_ctr_layout(t->max_rec_bytes, (uint32_t)t->max_rows, (uint32_t)t->max_chunks, (uint32_t)q.T, agg_mode, t->any_nonconst_ts);
-    const size_t cap = std::min<size_t>(ctx->max_smem_optin, 227 * 1024) - sizeof(TileCtrTab) * (TILE_CTR_TABMAX + 1) - 64;
-    size_t w = cap / W.per_warp; if (w > (size_t)WP_CTR_MAX_WARPS) w = WP_CTR_MAX_WARPS;
-    if (W.tsr != 0 && w > 16) w = 16;                     // the irregular-timestamp instantiation is built for <= 16 warps
-    static const int warps_env = [] { const char* e = std::getenv("FILO_WP_WARPS"); return e ? atoi(e) : 0; }();
-    if (warps_env > 0 && (size_t)warps_env < w) w = (size_t)warps_env;
-    if (w < 4) return false;
-    W.warps = (uint32_t)w; W.tab = (uint32_t)(W.per_warp * w);
-    return true;
-  };
+  // v4 counter-class kernel (scan_wp_ctr.cuh): per-series rows, or fused partial rows of up to TILE_AGG_ACC * TILE_THREADS windows;
+  // what it declines goes to the v2 kernel
+  WpCtrSmem WC{};
+  bool use_wp_ctr = false;
+  if (use_v2 && force != "v2" && force != "v3" && fn_cls == CLASS_COUNTER && t->n_series > 0 && t->max_chunks > 0 &&
+      (!fused || q.T <= TILE_AGG_ACC * TILE_THREADS) && wp_ctr_tile_footprint_ok(t->max_rec_bytes, (uint32_t)t->max_rows, (uint32_t)q.T, smem_cap)) {
+    WC = wp_ctr_layout(t->max_rec_bytes, (uint32_t)t->max_rows, (uint32_t)t->max_chunks, (uint32_t)q.T, fused, t->any_nonconst_ts);
+    // the irregular-timestamp instantiation is built for <= 16 warps
+    const size_t w = std::min<size_t>((smem_cap - sizeof(TileCtrTab) * (TILE_CTR_TABMAX + 1) - 64) / WC.per_warp, WC.tsr != 0 ? 16 : WP_CTR_MAX_WARPS);
+    WC.warps = (uint32_t)w; WC.tab = (uint32_t)(WC.per_warp * w);
+    use_wp_ctr = w >= 4;
+  }
   auto run_per_series = [&](double* outp) -> int32_t {
-    if (use_tile) {
+    if (use_tile || use_wp_ctr) {
       int64_t* d_list = nullptr; unsigned long long* d_cnt = nullptr;
       CUDA_TRY(ctx, tmp.alloc((void**)&d_list, (size_t)t->n_series * 8));
       CUDA_TRY(ctx, tmp.alloc((void**)&d_cnt, 16));
       CUDA_TRY(ctx, cudaMemsetAsync(d_cnt, 0, 16, s));
       ScanLaunch LT = L;
-      const int ctas_per_sm = ((size_t)TL.total + 1024) * 2 <= (size_t)228 * 1024 ? 2 : 1;
-      const int64_t n_tiles = (t->n_series + TILE_NS - 1) / TILE_NS;
-      LT.grid = (int)std::max<int64_t>(1, std::min<int64_t>(n_tiles, (int64_t)ctx->sm_count * ctas_per_sm));
       static const bool dbg = std::getenv("FILO_DEBUG_SYNC") != nullptr;
-      if (dbg) { fprintf(stderr, "[filo] tile kernel fn=%d T=%d grid=%d smem=%u pitch=%u\n", fn, q.T, LT.grid, TL.total, TL.vals_pitch); fflush(stderr); }
-      WpCtrSmem WC;
       if (use_wp) {
         LT.grid = (int)std::max<int64_t>(1, std::min<int64_t>((t->n_series + WL.warps - 1) / WL.warps, (int64_t)ctx->sm_count));
         CUDA_TRY(ctx, launch_scan_wp(LT, outp, WL, d_list, d_cnt));
-      } else if (wp_ctr_plan(false, WC)) {
+      } else if (use_wp_ctr) {
         LT.grid = (int)std::max<int64_t>(1, std::min<int64_t>((t->n_series + WC.warps - 1) / WC.warps, (int64_t)ctx->sm_count));
         CUDA_TRY(ctx, launch_scan_wp_ctr(LT, outp, WC, d_list, d_cnt));
-      } else CUDA_TRY(ctx, launch_scan_tile(LT, outp, TL, d_list, d_cnt));
+      } else {
+        const int ctas_per_sm = ((size_t)TL.total + 1024) * 2 <= (size_t)228 * 1024 ? 2 : 1;
+        const int64_t n_tiles = (t->n_series + TILE_NS - 1) / TILE_NS;
+        LT.grid = (int)std::max<int64_t>(1, std::min<int64_t>(n_tiles, (int64_t)ctx->sm_count * ctas_per_sm));
+        if (dbg) { fprintf(stderr, "[filo] tile kernel fn=%d T=%d grid=%d smem=%u pitch=%u\n", fn, q.T, LT.grid, TL.total, TL.vals_pitch); fflush(stderr); }
+        CUDA_TRY(ctx, launch_scan_tile(LT, outp, TL, d_list, d_cnt));
+      }
       if (dbg) { CUDA_TRY(ctx, cudaStreamSynchronize(s)); fprintf(stderr, "[filo] tile kernel done\n"); fflush(stderr); }
       ScanLaunch LF = L; LF.list = d_list; LF.list_count = d_cnt;
       CUDA_TRY(ctx, launch_scan_series_v2(LF, outp, rec_cap_used));
@@ -994,20 +975,21 @@ static int32_t query_device_impl(filo_ctx* ctx, const filo_table* t, int32_t fn,
     CUDA_TRY(ctx, tmp.alloc((void**)&pval, (size_t)t->n_items * q.T * 8));
     CUDA_TRY(ctx, tmp.alloc((void**)&pcnt, (size_t)t->n_items * q.T * 4));
     const int32_t* order = t->grouped ? t->d_order : nullptr;
-    if (use_tile && q.T <= TILE_AGG_ACC * TILE_THREADS) {
-      // tile kernel folds every item into one partial row; items with a series it declines go through the v2 kernel
+    if ((use_tile && q.T <= TILE_AGG_ACC * TILE_THREADS) || use_wp_ctr) {
+      // the tile / v4 counter kernel folds every item into one partial row; items with a series it declines go through the v2 kernel
       int64_t* d_list = nullptr; unsigned long long* d_cnt = nullptr;
       CUDA_TRY(ctx, tmp.alloc((void**)&d_list, (size_t)t->n_items * 8));
       CUDA_TRY(ctx, tmp.alloc((void**)&d_cnt, 16));
       CUDA_TRY(ctx, cudaMemsetAsync(d_cnt, 0, 16, s));
       ScanLaunch LT = L;
-      const int ctas_per_sm = ((size_t)TL.total + 1024) * 2 <= (size_t)228 * 1024 ? 2 : 1;
-      LT.grid = (int)std::max<int64_t>(1, std::min<int64_t>(t->n_items, (int64_t)ctx->sm_count * ctas_per_sm));
-      WpCtrSmem WC;
-      if (wp_ctr_plan(true, WC)) {
+      if (use_wp_ctr) {
         LT.grid = (int)std::max<int64_t>(1, std::min<int64_t>((t->n_items + WC.warps - 1) / WC.warps, (int64_t)ctx->sm_count));
         CUDA_TRY(ctx, launch_scan_wp_ctr_agg(LT, WC, order, t->d_item_begin, t->n_items, agg, pval, pcnt, d_list, d_cnt));
-      } else CUDA_TRY(ctx, launch_scan_tile_agg(LT, TL, order, t->d_item_begin, t->n_items, agg, pval, pcnt, d_list, d_cnt));
+      } else {
+        const int ctas_per_sm = ((size_t)TL.total + 1024) * 2 <= (size_t)228 * 1024 ? 2 : 1;
+        LT.grid = (int)std::max<int64_t>(1, std::min<int64_t>(t->n_items, (int64_t)ctx->sm_count * ctas_per_sm));
+        CUDA_TRY(ctx, launch_scan_tile_agg(LT, TL, order, t->d_item_begin, t->n_items, agg, pval, pcnt, d_list, d_cnt));
+      }
       ScanLaunch LF = L; LF.list = d_list; LF.list_count = d_cnt;
       CUDA_TRY(ctx, launch_scan_agg_v2(LF, order, t->d_item_begin, t->n_items, agg, pval, pcnt, acc_bytes, rec_cap_used));
       launches += 1;

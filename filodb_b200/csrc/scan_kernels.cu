@@ -434,36 +434,23 @@ cudaError_t launch_scan_agg_v2(const ScanLaunch& L, const int32_t* order, const 
   }
 }
 struct TileAggArgs { const int32_t* order; const int64_t* item_begin; int64_t n_items; int agg_op; double* pval; uint32_t* pcnt; };
-template <int CLS, int FN, bool AGG, int DEC>
-static cudaError_t launch_tile_dec(const ScanLaunch& L, double* out, const TileSmem& T, int64_t* fallback_list, unsigned long long* fallback_count,
-                                   const TileAggArgs& A) {
-  cudaError_t e = cudaFuncSetAttribute(scan_tile_kernel<CLS, FN, AGG, DEC>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)T.total);
-  if (e != cudaSuccess) return e;
-  scan_tile_kernel<CLS, FN, AGG, DEC><<<L.grid, TILE_LAUNCH_THREADS, T.total, L.stream>>>(L.arena, L.rec_off, L.n_series, L.q, out, T, fallback_list, fallback_count,
-      L.d_counters, L.d_err, A.order, A.item_begin, A.n_items, A.agg_op, A.pval, A.pcnt);
-  return cudaGetLastError();
-}
-template <int CLS, int FN, bool AGG>
+template <int FN, bool AGG>
 static cudaError_t launch_tile_fn(const ScanLaunch& L, double* out, const TileSmem& T, int64_t* fallback_list, unsigned long long* fallback_count,
                                   const TileAggArgs& A) {
-  if (T.opts & TILE_OPT_WARPDEC) return launch_tile_dec<CLS, FN, AGG, 1>(L, out, T, fallback_list, fallback_count, A);      // experimental per-warp decode
-  return launch_tile_dec<CLS, FN, AGG, 0>(L, out, T, fallback_list, fallback_count, A);
+  cudaError_t e = cudaFuncSetAttribute(scan_tile_kernel<FN, AGG>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)T.total);
+  if (e != cudaSuccess) return e;
+  scan_tile_kernel<FN, AGG><<<L.grid, TILE_LAUNCH_THREADS, T.total, L.stream>>>(L.arena, L.rec_off, L.n_series, L.q, out, T, fallback_list, fallback_count,
+      L.d_counters, L.d_err, A.order, A.item_begin, A.n_items, A.agg_op, A.pval, A.pcnt);
+  return cudaGetLastError();
 }
 template <bool AGG>
 static cudaError_t launch_tile_any(const ScanLaunch& L, double* out, const TileSmem& T, int64_t* fallback_list, unsigned long long* fallback_count,
                                    const TileAggArgs& A) {
-  if (fn_class_of(L.q.fn, L.q.cumulative, L.q.long_values) == CLASS_COUNTER) {
-    switch (L.q.fn) {
-      case FN_RATE: return launch_tile_fn<CLASS_COUNTER, FN_RATE, AGG>(L, out, T, fallback_list, fallback_count, A);
-      case FN_INCREASE: return launch_tile_fn<CLASS_COUNTER, FN_INCREASE, AGG>(L, out, T, fallback_list, fallback_count, A);
-      default: return launch_tile_fn<CLASS_COUNTER, FN_DELTA, AGG>(L, out, T, fallback_list, fallback_count, A);
-    }
-  }
   switch (L.q.fn) {
-    case FN_RATE: return launch_tile_fn<CLASS_SUM, FN_RATE, AGG>(L, out, T, fallback_list, fallback_count, A);
-    case FN_AVG: return launch_tile_fn<CLASS_SUM, FN_AVG, AGG>(L, out, T, fallback_list, fallback_count, A);
-    case FN_COUNT: return launch_tile_fn<CLASS_SUM, FN_COUNT, AGG>(L, out, T, fallback_list, fallback_count, A);
-    default: return launch_tile_fn<CLASS_SUM, FN_SUM, AGG>(L, out, T, fallback_list, fallback_count, A);      // FN_SUM, FN_INCREASE on a delta schema
+    case FN_RATE: return launch_tile_fn<FN_RATE, AGG>(L, out, T, fallback_list, fallback_count, A);
+    case FN_AVG: return launch_tile_fn<FN_AVG, AGG>(L, out, T, fallback_list, fallback_count, A);
+    case FN_COUNT: return launch_tile_fn<FN_COUNT, AGG>(L, out, T, fallback_list, fallback_count, A);
+    default: return launch_tile_fn<FN_SUM, AGG>(L, out, T, fallback_list, fallback_count, A);      // FN_SUM, FN_INCREASE on a delta schema
   }
 }
 cudaError_t launch_scan_tile(const ScanLaunch& L, double* out, const TileSmem& T, int64_t* fallback_list, unsigned long long* fallback_count) {

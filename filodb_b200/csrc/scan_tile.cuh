@@ -1,4 +1,6 @@
-// v3 scan path: CTA-tile kernel for the regular case (the BASELINE workloads).
+// v3 scan path: CTA-tile kernel for the SUM class (sum / avg / count_over_time, rate / increase on delta schemas) over regular series.
+// It serves the fused across-series aggregates (the v4 kernel of scan_wp.cuh has no aggregate mode) and the per-series queries the v4
+// SUM kernel turns away (windows over more than 4096 rows, fewer than 4 warps in shared memory).
 //
 // A CTA processes tiles of TILE_NS consecutive series.  Records of consecutive series are adjacent in the arena, so a tile's
 // chunk pages arrive with ONE cp.async.bulk (TMA) into shared memory, and the tile's [TILE_NS x T] results leave with ONE
@@ -20,8 +22,6 @@
 namespace filo {
 
 #ifdef FILO_CUSIM
-#define FILO_NOINLINE __attribute__((noinline))
-inline long cusim_junction_blocks = 0, cusim_rest_windows = 0;
 inline void tma_store_1d(void* gdst, const void* ssrc, uint32_t bytes) { cusim::tma_store(gdst, ssrc, bytes); }
 inline void tma_store_wait_read() { cusim::tma_store_wait_read(); }
 inline void fence_async_smem() {}
@@ -32,7 +32,6 @@ __device__ __forceinline__ void tma_store_1d(void* gdst, const void* ssrc, uint3
 }
 __device__ __forceinline__ void tma_store_wait_read() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
 __device__ __forceinline__ void fence_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-#define FILO_NOINLINE __noinline__
 #endif
 
 // Per-phase cycle counters of the consumer side for profiling builds (-DFILO_TILE_PROF; scratch/tile_prof.py): lane 0 of every
@@ -88,159 +87,13 @@ __device__ __forceinline__ double tile_eval_window(const TileSeries& S, const do
   return sum;
 }
 
-__device__ __forceinline__ double nan0(double x) { return x != x ? 0.0 : x; }
-// correction accumulated up to and including row r.  The list has been sorted by position and its amounts replaced by their
-// running sums in position order (tile kernel, start of the window phase) -- the same additions as the reference's running
-// `_correction += last` -- so the answer is the entry of the last drop at or before r.
-__device__ __forceinline__ double drops_cum(const TileDrops& D, int r) {
-  const int n = D.n < TILE_MAXDROP ? D.n : TILE_MAXDROP;
-  double cum = 0.0;
-#pragma unroll
-  for (int j = 0; j < TILE_MAXDROP; ++j) if (j < n && D.pos[j] <= r) cum = D.amt[j];
-  return cum;
-}
-// value of row r as the counter functions see it: CorrectingDoubleVectorReader.corrected for a drop-flagged chunk, raw otherwise
-__device__ __forceinline__ double ctr_value(const double* v, int r, const TileDrops& D, bool dropped) {
-  const double x = v[r];
-  if (!dropped) return x;
-  return nan0(x) + drops_cum(D, r);
-}
-
-// RateFunctions.extrapolatedRate (RateFunctions.scala:72-111), same operations in the same order; the divisions by the constants
-// 1000 and (windowEnd - windowStart) use the exact invariant-divisor sequence, and the zero-point quotient is only formed
-// when durationToZero can be below durationToStart: v1 * sI > 2 * dTS * delta  =>  sI * (v1 / delta) >= dTS
-template <bool IS_COUNTER, bool IS_RATE>
-__device__ __forceinline__ double extrapolated_rate_tile(int64_t windowStart, int64_t windowEnd, int32_t numSamples, int64_t t1, double v1,
-                                                         int64_t t2, double v2, double fdiv, double frcp, int64_t step, const TileCtrTab* tab) {
-  double durationToStart = div_invariant((double)(t1 - windowStart), 1000.0, 0.001);
-  const double durationToEnd = div_invariant((double)(windowEnd - t2), 1000.0, 0.001);
-  const int64_t si_ms = t2 - t1;
-  const int m = numSamples - 1;
-  double sampledInterval, extrapolationThreshold, half, rcpSI;
-  if (m <= TILE_CTR_TABMAX && si_ms == (int64_t)m * step) {      // samples m steps apart: the terms depend on m only (see the table)
-    const TileCtrTab e = tab[m];
-    sampledInterval = e.sI; extrapolationThreshold = e.thr; half = e.half; rcpSI = e.rcpSI;
-  } else {
-    sampledInterval = div_invariant((double)si_ms, 1000.0, 0.001);
-    const double averageDurationBetweenSamples = ddiv_rare(sampledInterval, (double)numSamples - 1.0);
-    extrapolationThreshold = averageDurationBetweenSamples * 1.1; half = averageDurationBetweenSamples / 2.0; rcpSI = 0.0;
-  }
-  const double delta = v2 - v1;
-  if (IS_COUNTER && delta > 0 && v1 >= 0) {
-    if (!(v1 * sampledInterval > 2.0 * durationToStart * delta)) {
-      const double durationToZero = sampledInterval * ddiv_rare(v1, delta);
-      if (durationToZero < durationToStart) durationToStart = durationToZero;
-    }
-  }
-  double extrapolateToInterval = sampledInterval;
-  extrapolateToInterval += (durationToStart < extrapolationThreshold) ? durationToStart : half;
-  extrapolateToInterval += (durationToEnd < extrapolationThreshold) ? durationToEnd : half;
-  const double ratio = rcpSI != 0.0 ? div_invariant(extrapolateToInterval, sampledInterval, rcpSI) : ddiv_rare(extrapolateToInterval, sampledInterval);
-  const double scaledDelta = delta * ratio;
-  return IS_RATE ? __dmul_rn(div_invariant(scaledDelta, fdiv, frcp), 1000.0) : scaledDelta;
-}
-
-// literal per-chunk fold of the counter functions for one window of a regular series: CounterChunkedRangeFunction.addChunks
-// (RangeFunction.scala:131-172), ChunkedRateFunctionBase (RateFunctions.scala:230-285), correction carry
-// (DoubleVector.scala:177-207, 375-391).
-template <int FN>
-__device__ __forceinline__ double tile_eval_counter(const TileSeries& S, const TileCtr* K, const TileDrops* DR, const double* vals, const QueryParams& q,
-                                                    int64_t wStart, int64_t wEnd, int k, double fdiv, double frcp, const TileCtrTab* tab) {
-  const double NaNv = __longlong_as_double(0x7ff8000000000000LL);
-  int32_t numSamples = 0; int64_t loT = INT64_MAX, hiT = 0; double loV = NaNv, hiV = NaNv;
-  bool some = false; double corrLast = 0.0, corr = 0.0;                // correctionMeta
-  for (int c = 0; c < S.n; ++c) {
-    const TileChunk& ch = S.c[c];
-    if (ch.end_time < wStart) continue;                                // ChunkSetInfo.scala:481-510
-    if (c > 0 && !(S.c[c - 1].end_time < wEnd)) continue;
-    int su = ch.s0 + k; if (su < 0) su = 0;
-    int eu = ch.e0 + k; if (eu > ch.nrows - 1) eu = ch.nrows - 1;
-    const double* v = vals + ch.row_base;
-    const double first = __longlong_as_double((long long)ch.first);
-    if (FN != FN_DELTA && some) { if (first != first || first < corrLast) corr = corr + corrLast; }
-    if (su <= eu) {
-      const int64_t tS = ch.init + (int64_t)su * q.step, tE = ch.init + (int64_t)eu * q.step;
-      const bool skip = FN != FN_DELTA && su == 0 && eu == 0 && first != first;      // RateFunctions.scala:255-256
-      if (!skip && (tS < loT || tE > hiT)) {
-        numSamples += eu - su + 1;
-        const bool drp = FN != FN_DELTA && K[c].dropped;
-        if (tS < loT) { loT = tS; const double b = ctr_value(v, su, DR[c], drp); loV = (FN != FN_DELTA && some) ? b + corr : b; }
-        if (tE > hiT) { hiT = tE; const double b = ctr_value(v, eu, DR[c], drp); hiV = (FN != FN_DELTA && some) ? b + corr : b; }
-      }
-    }
-    if (FN != FN_DELTA) {
-      if (K[c].dropped) {                                                // CorrectingDoubleVectorReader.updateCorrection, :375-391
-        int idx = ch.vlen - 1; double lastValue = 0.0;
-        do { lastValue = v[idx]; idx -= 1; } while (lastValue != lastValue && idx >= 0);
-        corrLast = nan0(lastValue); corr = (some ? corr : 0.0) + drops_cum(DR[c], ch.vlen - 1);
-      }
-      else { corrLast = v[ch.vlen - 1]; corr = some ? corr : 0.0; }
-    }
-    some = true;
-  }
-  const int64_t cws = q.inclusive ? wStart : wStart - 1;               // RateFunctions.scala:270-285
-  if (hiT > loT) return extrapolated_rate_tile<FN != FN_DELTA, FN == FN_RATE>(cws, wEnd, numSamples, loT, loV, hiT, hiV, fdiv, frcp, q.step, tab);
-  return NaNv;
-}
-
-// One block of JUNC_R windows of the junction between chunk c-1 and chunk c of a regular series (SUM class): each window's rows lie
-// in those two chunks only, both are members of its chunk set (the producer checked), so the window is the per-chunk fold of
-// tile_eval_window with the two chunk sums computed JUNC_R windows at a time.  JUNC_R is about half of BLK_R: a junction block (two
-// partial sums) then costs about as much as a regular block (one sum of BLK_R windows), which keeps the tile's work items even.
-// A tile with NaN / Inf rows takes the literal fold.
-constexpr int JUNC_R = 8;
-template <int FN>
-__device__ FILO_NOINLINE void tile_junction_block(const TileSeries& S, int c, const double* sv, double* orow, int jb, bool any_nan, const QueryParams& q,
-                                                 int64_t winDur, double fdiv, double frcp) {
-  const TileChunk& cb = S.c[c]; const TileChunk& ca = S.c[c - 1];
-#ifdef FILO_CUSIM
-  ++cusim_junction_blocks;          // emulation statistics (tests/cpp/tile_emul.cpp)
-#endif
-  const int k0 = cb.jk0 + jb * JUNC_R;
-  int nw = cb.jk0 + cb.jn - k0; if (nw > JUNC_R) nw = JUNC_R;
-  double* o = orow + k0;
-  if (any_nan) {
-    for (int j = 0; j < nw; ++j) {
-      const int64_t wEnd = q.start + (int64_t)(k0 + j) * q.step;
-      o[j] = tile_eval_window<FN, true>(S, sv, wEnd - winDur, wEnd, fdiv, k0 + j);
-    }
-    return;
-  }
-  const double NaNv = __longlong_as_double(0x7ff8000000000000LL);
-  double acc[JUNC_R]; int cnt[JUNC_R];
-  blocked_sum_r<JUNC_R, false, true, true>(sv + ca.row_base, ca.s0 + k0, ca.nrows, ca.Wr, acc, cnt);
-#pragma unroll
-  for (int j = 0; j < JUNC_R; ++j) if (j < nw) o[j] = acc[j];        // chunk c-1's sums wait in the window's own output slot
-  blocked_sum_r<JUNC_R, false, true, true>(sv + cb.row_base, cb.s0 + k0, cb.nrows, cb.Wr, acc, cnt);
-#pragma unroll
-  for (int j = 0; j < JUNC_R; ++j) {
-    if (j < nw) {
-      int lo = ca.s0 + k0 + j; if (lo < 0) lo = 0;
-      int hi = ca.s0 + k0 + j + ca.Wr; if (hi > ca.nrows - 1) hi = ca.nrows - 1;
-      const int na = hi >= lo ? hi - lo + 1 : 0, nb = cnt[j];
-      double sum = NaNv;                                              // AggrOverTimeFunctions.scala:560-571, chunk by chunk
-      if (na) { sum = 0.0; sum += o[j]; }
-      if (nb) { if (sum != sum) sum = 0.0; sum += acc[j]; }
-      const int nn = na + nb;
-      double r;
-      if (FN == FN_RATE) r = __dmul_rn(div_invariant(sum, fdiv, frcp), 1000.0);
-      else if (FN == FN_AVG) r = nn > 0 ? sum / (double)nn : (sum != sum ? sum : 0.0);
-      else if (FN == FN_COUNT) r = nn > 0 ? (double)nn : NaNv;
-      else r = sum;
-      o[j] = r;
-    }
-  }
-}
-
 __device__ __forceinline__ uint64_t shfl_u64(uint64_t v, int src) { return (uint64_t)__shfl_sync(0xffffffffu, (unsigned long long)v, src); }
 __device__ __forceinline__ uint64_t shfl_up_u64(uint64_t v, int d) { return (uint64_t)__shfl_up_sync(0xffffffffu, (unsigned long long)v, d); }
 
 // ---------------------------------------------------------------------------------------------------------------------
-// Tile kernel, no across-series aggregate.  CLS = CLASS_SUM: sum/avg/count_over_time, rate/increase on delta schemas;
-// CLS = CLASS_COUNTER: rate/increase on cumulative schemas (counter correction) and delta.
+// Tile kernel: sum/avg/count_over_time, rate/increase on delta schemas.  AGG: fused across-series aggregate (partial rows).
 // ---------------------------------------------------------------------------------------------------------------------
-// DEC = 1 (TILE_OPT_WARPDEC): warp w decodes series w alone -- see the decode block
-template <int CLS, int FN, bool AGG, int DEC = 0>
+template <int FN, bool AGG>
 __global__ void __launch_bounds__(TILE_LAUNCH_THREADS, 2)
 scan_tile_kernel(const uint8_t* __restrict__ arena, const int64_t* __restrict__ rec_off, int64_t n_series,
                      QueryParams q, double* __restrict__ out, TileSmem L,
@@ -294,7 +147,6 @@ scan_tile_kernel(const uint8_t* __restrict__ arena, const int64_t* __restrict__ 
     for (bool more = walk_start(w); more; more = walk_next(w), b ^= 1) {
       TileSeries* SDn = reinterpret_cast<TileSeries*>(smem + L.desc + b * L.desc_stride);
       TileMeta* Mn = reinterpret_cast<TileMeta*>(smem + L.meta + b * 128);
-      TileCtr* CTn = reinterpret_cast<TileCtr*>(smem + L.ctr) + b * (TILE_NS * TILE_MAXC);
       const int64_t i0 = w.pb;
       const int ns = (int)(w.pe - w.pb < TILE_NS ? w.pe - w.pb : TILE_NS);
       // lanes 0..ns-1: series id, record offset and size; records land back to back in the staging buffer
@@ -334,13 +186,12 @@ scan_tile_kernel(const uint8_t* __restrict__ arena, const int64_t* __restrict__ 
       }
       const ChunkEntry* E = reinterpret_cast<const ChunkEntry*>(rec + sizeof(RecordHeader)) + cLo;
       bool have = regular && c < n;
-      int64_t init = 0, end_time = 0; int tlen = 0, vlen = 0, ng = 0, vwire = 0, nrows = 0, num_rows = 0, vbytes = 0, dropped = 0; uint32_t voff = 0, w12 = 0;
+      int64_t init = 0, end_time = 0; int tlen = 0, vlen = 0, ng = 0, vwire = 0, nrows = 0, num_rows = 0, vbytes = 0; uint32_t voff = 0, w12 = 0;
       bool okc = true;
       if (have) {
         const ChunkEntry& e = E[c];
         const uint8_t* tv = rec + e.ts_off; const uint8_t* vv = rec + e.val_off;
-        const uint32_t vw4 = ld32(vv + 4);
-        vwire = vw4 & 0xffff; dropped = (vw4 >> 31) & 1;       // PrimitiveVectorReader.dropped, BinaryVector.scala:530-531
+        vwire = ld32(vv + 4) & 0xffff;
         tlen = (int)ld32(tv + 8); init = (int64_t)ld64_a4(tv + 12); const int slope = (int)ld32(tv + 20);
         end_time = e.end_time; num_rows = e.num_rows; voff = roff + e.val_off;
         vbytes = (int)ld32(tv) + 4 + (int)ld32(vv) + 4;
@@ -349,7 +200,6 @@ scan_tile_kernel(const uint8_t* __restrict__ arena, const int64_t* __restrict__ 
         else okc = false;
         if ((int64_t)slope != q.step || tlen <= 0 || vlen <= 0) okc = false;
         nrows = num_rows < tlen ? num_rows : tlen; if (vlen < nrows) nrows = vlen;
-        if (CLS == CLASS_COUNTER && vlen != nrows) okc = false;     // updateCorrection reads the vector's last element
       }
       const unsigned okm = __ballot_sync(0xffffffffu, okc);     // (not inside the &&: every lane must take part)
       regular = regular && ((okm >> lb) & 0xfu) == 0xfu;
@@ -380,93 +230,39 @@ scan_tile_kernel(const uint8_t* __restrict__ arena, const int64_t* __restrict__ 
       if (v4 < kB) kB = v4;
       if (kA < 0) kA = 0;
       if (kB > q.T - 1) kB = q.T - 1;
-      const int64_t kA2 = kA, kB2 = kB;    // every single-chunk window of the chunk
-      if (CLS == CLASS_COUNTER) {          // [kA, kB]: only windows whose row range is not clamped by the chunk's ends
-        if (-s0 > kA) kA = -s0;
-        const int64_t x = (int64_t)(nrows - 1) - e0; if (x < kB) kB = x;
-      }
       const int64_t sA = s0 + kA, eA = e0 + kA;
       const bool ok = have && kA <= kB && eA >= sA;
       const int Wr = ok ? (int)(eA - sA) : 0;
       const int nwin = ok ? (int)(kB - kA + 1) : 0;
       // blocked only when the windows are long enough to amortise a block; short windows go through the per-window path
-      // COUNTER: work item = one window of the interval (needs two samples: Wr >= 1)
-      const bool blocked = ok && Wr >= (CLS == CLASS_COUNTER ? 1 : BLK_R - 1);
-      const int nb = !blocked ? 0 : (CLS == CLASS_COUNTER ? nwin : (nwin + BLK_R - 1) / BLK_R);
-      // SUM class: junction with the previous chunk.  The windows between the two blocked intervals take rows from both chunks;
-      // they go through two blocked partial sums instead of the per-window fold when (a) both chunks are members of every such
-      // window's chunk set (ChunkSetInfo.scala:481-510) and (b) no other chunk has a row in them
-      int jk0 = 0, jn = 0, jb = 0;
-      {
-        const int blocked_p = __shfl_up_sync(0xffffffffu, blocked ? 1 : 0, 1);
-        const int64_t kBp = __shfl_up_sync(0xffffffffu, kB, 1);
-        const int64_t s0pp = __shfl_up_sync(0xffffffffu, s0, 2), endpp = __shfl_up_sync(0xffffffffu, end_time, 2);
-        const int nrowspp = __shfl_up_sync(0xffffffffu, nrows, 2);
-        if (CLS == CLASS_SUM && (L.opts & TILE_OPT_JUNCTION) && c > 0 && blocked && blocked_p) {
-          const int64_t gapA = kBp + 1, gapB = kA - 1, n_gap = gapB - gapA + 1;
-          const int64_t wStartB = S0 + gapB * q.step, wEndA = E0 + gapA * q.step;
-          bool okj = n_gap >= 1 && n_gap <= 4 * JUNC_R && Wr >= JUNC_R - 1;
-          okj = okj && !(endp < wStartB) && endp < wEndA && !(end_time < wStartB);                 // both chunks in the chunk set of every gap window
-          if (c >= 2) okj = okj && endpp < wEndA && s0pp + gapA > (int64_t)nrowspp - 1;             // chunk c-2: out of the rows
-          if (c + 1 < n) okj = okj && e0n + gapB < 0;                                               // chunk c+1: not reached yet
-          if (okj) { jk0 = (int)gapA; jn = (int)n_gap; jb = (jn + JUNC_R - 1) / JUNC_R; }
-        }
-      }
+      const bool blocked = ok && Wr >= BLK_R - 1;
+      const int nb = blocked ? (nwin + BLK_R - 1) / BLK_R : 0;
       // zero rows around the chunk so that blocked sums read clamped-away rows as +0.0 without a bounds check
       int lowz = 0, highz = 0;
-      if (blocked && CLS == CLASS_SUM) {
+      if (blocked) {
         if (sA < 0) lowz = (int)-sA;
         const int64_t over = sA + (nwin - 1) + Wr - (nrows - 1); if (over > 0) highz = (int)over;
       }
       int need = 0;
       (void)xpre(lowz + nrows + highz, need);
-      const bool padded = need + BLK_R + (DEC ? TILE_MAXC : 0) <= (int)L.vals_pitch;
+      const bool padded = need + BLK_R <= (int)L.vals_pitch;
       if (!padded) { lowz = 0; highz = 0; }
-      if (DEC) {
-        // 16-byte row stores: every chunk's rows start at an odd offset of the (even-pitch) series row, so that row 1 -- the first row
-        // of its first group -- is 16-byte aligned.  One extra zero row in front of a chunk fixes the parity; chunks in order.
-        const int t_c = have ? lowz + nrows + highz : 0;
-        const int t0 = __shfl_sync(0xffffffffu, t_c, lb), t1 = __shfl_sync(0xffffffffu, t_c, lb + 1), t2 = __shfl_sync(0xffffffffu, t_c, lb + 2);
-        const int l0 = __shfl_sync(0xffffffffu, lowz, lb), l1 = __shfl_sync(0xffffffffu, lowz, lb + 1), l2 = __shfl_sync(0xffffffffu, lowz, lb + 2), l3 = __shfl_sync(0xffffffffu, lowz, lb + 3);
-        const int e0p = ((l0) & 1) ? 0 : 1;                              // chunk 0: row_base = lowz0 (+ e)
-        const int b1 = t0 + e0p, e1p = ((b1 + l1) & 1) ? 0 : 1;
-        const int b2 = b1 + t1 + e1p, e2p = ((b2 + l2) & 1) ? 0 : 1;
-        const int b3 = b2 + t2 + e2p, e3p = ((b3 + l3) & 1) ? 0 : 1;
-        if (have) lowz += c == 0 ? e0p : c == 1 ? e1p : c == 2 ? e2p : e3p;
-      }
       int nrows_tot = 0;
       const int row_base = xpre(lowz + nrows + highz, nrows_tot) + lowz;
       if (ngroups > TILE_MAXG || nrows_tot + 2 > (int)L.vals_pitch) { regular = false; have = false; }
       int nblocks = 0, covered = 0;
-      const int blk0 = xpre(have ? nb + jb : 0, nblocks); (void)xpre(have && blocked ? nwin + jn : 0, covered);
+      const int blk0 = xpre(have ? nb : 0, nblocks); (void)xpre(have && blocked ? nwin : 0, covered);
       int cnt_rows = 0, cnt_bytes = 0;            // this chunk's contribution to the scan counters
       if (have) {
         TileChunk& ch = S.c[c];
         ch.init = init; ch.end_time = end_time; ch.nrows = nrows; ch.row_base = row_base;
-        ch.val_off = voff; ch.wire = vwire; ch.ngroups = ng; ch.grp_base = grp_base; ch.tlen = tlen; ch.vlen = vlen;
-        ch.kA2 = (have && kA2 <= kB2) ? (int)kA2 : 0; ch.kB2 = (have && kA2 <= kB2) ? (int)kB2 : -1;
+        ch.val_off = voff; ch.wire = vwire; ch.ngroups = ng; ch.grp_base = grp_base;
         ch.kA = blocked ? (int)kA : 0; ch.kB = blocked ? (int)kB : -1; ch.sA = (int)sA; ch.Wr = Wr; ch.blk0 = blk0; ch.blk_n = nb;
-        ch.jk0 = jk0; ch.jn = jn; ch.jblk = jb; ch.kAj = jb ? jk0 : ch.kA;
         ch.s0 = (int)s0; ch.e0 = (int)e0;
         if (vwire == WIRE_XOR) {
           const uint32_t po = w12 >> 16;
           ch.first = ld64(recbuf + voff + po); ch.grp_off = voff + po + 8; ch.tab_off = voff + XOR_OFF_GROUPTAB;
         } else { ch.first = ld64(recbuf + voff + 8); ch.grp_off = 0; ch.tab_off = 0; }
-        if (CLS == CLASS_COUNTER) {
-          // RateFunctions.extrapolatedRate (RateFunctions.scala:72-111) for the chunk's unclamped single-chunk windows: the
-          // sample times move with the window, so durationToStart/End, sampledInterval, numSamples are window-invariant
-          TileCtr& kc = CTn[s * TILE_MAXC + c];
-          kc.dropped = dropped;
-          if (blocked) {
-            const double dTS = (double)(init + s0 * q.step - S0 + (q.inclusive ? 0 : 1)) / 1000.0, dTE = (double)(E0 - (init + e0 * q.step)) / 1000.0;
-            const double sI = (double)((e0 - s0) * q.step) / 1000.0;
-            const double avg = sI / ((double)(Wr + 1) - 1.0), thr = avg * 1.1, half = avg / 2.0;
-            const double endpart = dTE < thr ? dTE : half;
-            const double eTI = (sI + (dTS < thr ? dTS : half)) + endpart;
-            kc.dTS = dTS; kc.thr = thr; kc.half = half; kc.endpart = endpart; kc.sI = sI; kc.ratio0 = eTI / sI;
-            kc.skipC = 2.0 * dTS / sI;      // v1 > delta * skipC  =>  durationToZero >= durationToStart (no zero-point clamp)
-          }
-        }
         ch.lowz = lowz; ch.highz = highz;          // zeroed by the consumers before they decode the tile
         // CountingChunkInfoIterator, ChunkSetInfo.scala:336-380: every chunk in range is pulled, except one that starts after
         // the last window end (the window iterator never reaches it)
@@ -479,7 +275,6 @@ scan_tile_kernel(const uint8_t* __restrict__ arena, const int64_t* __restrict__ 
       const unsigned irrm = __ballot_sync(0xffffffffu, present && !regular);
       if (AGG && irrm != 0) regular = false;      // an item is folded as a whole: one irregular series sends the item to the fallback
       const unsigned unpm = __ballot_sync(0xffffffffu, have && !padded);
-      const unsigned drpm = __ballot_sync(0xffffffffu, have && dropped);
       if (c == 0) {
         if (regular) {
           S.sid = sid; S.n = n; S.regular = 1; S.rec_off = (int)roff; S.nblocks = nblocks; S.nrest = q.T - covered; S.ngroups = ngroups; S.nrows = nrows_tot;
@@ -500,7 +295,7 @@ scan_tile_kernel(const uint8_t* __restrict__ arena, const int64_t* __restrict__ 
         if (lane >= o) { p += pp; r += rr; }
       }
       if (c == 0) { Mn->pref[s + 1] = p; Mn->rpref[s + 1] = r; }
-      if (lane == 0) { Mn->pref[0] = 0; Mn->rpref[0] = 0; Mn->any_nan = 0; Mn->any_raw = rawm != 0; Mn->all_regular = irrm == 0; Mn->all_padded = unpm == 0; Mn->any_drop = drpm != 0; Mn->staged = staged; Mn->ns = ns; Mn->i0 = i0; }
+      if (lane == 0) { Mn->pref[0] = 0; Mn->rpref[0] = 0; Mn->any_nan = 0; Mn->any_raw = rawm != 0; Mn->all_regular = irrm == 0; Mn->all_padded = unpm == 0; Mn->staged = staged; Mn->ns = ns; Mn->i0 = i0; }
       __syncwarp();
       if (lane == 0) mbar_arrive(ready + b);      // A(t): release the descriptors
       __syncthreads();          // B(t)
@@ -510,18 +305,6 @@ scan_tile_kernel(const uint8_t* __restrict__ arena, const int64_t* __restrict__ 
 
   // ==================================================================== consumer warps
   const bool out_aligned = (reinterpret_cast<uintptr_t>(out) & 15) == 0;
-  const TileCtrTab* CTAB = reinterpret_cast<const TileCtrTab*>(smem + L.tab);
-  if (CLS == CLASS_COUNTER) {
-    // extrapolation terms of RateFunctions.scala:74-77,92 for samples m steps apart: sampledInterval = (m * step) / 1000,
-    // averageDurationBetweenSamples = sampledInterval / (numSamples - 1) with numSamples - 1 = m
-    if (tid <= TILE_CTR_TABMAX) {
-      TileCtrTab& e = reinterpret_cast<TileCtrTab*>(smem + L.tab)[tid];
-      const double sI = (double)((int64_t)tid * q.step) / 1000.0;
-      const double avg = sI / ((double)(tid + 1) - 1.0);
-      e.sI = sI; e.thr = avg * 1.1; e.half = avg / 2.0; e.rcpSI = tid > 0 ? 1.0 / sI : 0.0;
-    }
-    bar_consumers();
-  }
   uint32_t parity = 0;
   int b = 0;
   double aacc[TILE_AGG_ACC]; uint32_t acnt[TILE_AGG_ACC]; bool item_bad = false;      // AGG: this thread's windows tid + j * TILE_THREADS
@@ -536,8 +319,6 @@ scan_tile_kernel(const uint8_t* __restrict__ arena, const int64_t* __restrict__ 
   for (bool more = walk_start(w); more; more = walk_next(w), b ^= 1) {
     const TileSeries* SDc = reinterpret_cast<const TileSeries*>(smem + L.desc + b * L.desc_stride);
     TileMeta* Mc = reinterpret_cast<TileMeta*>(smem + L.meta + b * 128);
-    TileCtr* CTc = reinterpret_cast<TileCtr*>(smem + L.ctr) + b * (TILE_NS * TILE_MAXC);
-    TileDrops* DRc = reinterpret_cast<TileDrops*>(smem + L.drops);
     TPROF(9)                                                // results of the previous tile (fold / store, loop overhead)
     mbar_wait_parked(ready + b, (tj >> 1) & 1); ++tj;   // A(t): descriptors ready (no consumer-wide barrier: the windows-end barrier of the
                                                  // previous tile already separates the tiles)
@@ -548,7 +329,6 @@ scan_tile_kernel(const uint8_t* __restrict__ arena, const int64_t* __restrict__ 
     if (warp == 0) {
       const TileSeries& S = SDc[lane >> 2];
       const int c = lane & 3;
-      if (CLS == CLASS_COUNTER) DRc[lane].n = 0;
       if (S.regular == 1 && c < S.n) {
         const TileChunk& ch = S.c[c];
         double* zr = vals + (size_t)(lane >> 2) * L.vals_pitch + ch.row_base;
@@ -560,15 +340,13 @@ scan_tile_kernel(const uint8_t* __restrict__ arena, const int64_t* __restrict__ 
     // Lane -> series lane & 7 (neighbouring lanes store to different series' rows: with the odd row pitch the 8-byte stores
     // of a warp spread over all banks); warp w owns the slots 8w .. 8w+7 of every series: item jj -> slot 8w + 4jj + (lane >> 3).
     {
-      // DEC = 1: warp w <-> series w, item jj -> slot 32 jj + lane: the whole XOR prefix stays inside the warp (no exchange through
-      // shared memory, no barrier); a lane's 8 rows leave as four 16-byte stores (lane stride 64 bytes: a quarter-warp covers all banks)
-      const int ds = DEC ? warp : (lane & 7);
+      const int ds = lane & 7;
       const TileSeries& S = SDc[ds];
       const bool sreg = S.regular == 1;
       uint64_t d[2][8]; uint64_t excl[2]; int cc[2]; bool act[2];
 #pragma unroll
       for (int jj = 0; jj < 2; ++jj) {
-        const int slot = DEC ? jj * 32 + lane : warp * 8 + jj * 4 + (lane >> 3);
+        const int slot = warp * 8 + jj * 4 + (lane >> 3);
         const bool active = sreg && slot < S.ngroups;
         const int c = (slot >= S.gb[1] ? 1 : 0) + (slot >= S.gb[2] ? 1 : 0) + (slot >= S.gb[3] ? 1 : 0);
         const TileChunk& ch = S.c[c];
@@ -599,26 +377,6 @@ scan_tile_kernel(const uint8_t* __restrict__ arena, const int64_t* __restrict__ 
         }
       }
       uint64_t pre0, pre1;
-      if (DEC) {
-        // inclusive XOR scan of the group totals over the 64 slots (item 0: slots 0..31, item 1: 32..63), then the exclusive
-        // prefixes go through a per-warp table so that a lane can look up the prefix at its chunk's first slot
-        uint64_t i0x = d[0][7], i1x = d[1][7];
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-          const uint64_t y0 = shfl_up_u64(i0x, o), y1 = shfl_up_u64(i1x, o);
-          if (lane >= o) { i0x ^= y0; i1x ^= y1; }
-        }
-        const uint64_t tot0 = shfl_u64(i0x, 31);
-        excl[0] = i0x ^ d[0][7]; excl[1] = i1x ^ d[1][7] ^ tot0;
-        uint64_t* wx = gexcl + warp * TILE_GX_PITCH;
-        wx[lane] = excl[0]; wx[32 + lane] = excl[1];
-        __syncwarp();
-        TPROF(1)
-        const TileChunk& c0 = S.c[cc[0]]; const TileChunk& c1 = S.c[cc[1]];
-        pre0 = c0.first ^ excl[0] ^ wx[act[0] ? c0.grp_base : 0];
-        pre1 = c1.first ^ excl[1] ^ wx[act[1] ? c1.grp_base : 0];
-        TPROF(2)
-      } else {
       // XOR of the group totals of earlier slots of the same series inside this warp (lanes ds, ds+8, ds+16, ds+24; item 0 first)
       uint64_t i0x = d[0][7], i1x = d[1][7];
       { const uint64_t y0 = shfl_up_u64(i0x, 8), y1 = shfl_up_u64(i1x, 8); if (lane >= 8) { i0x ^= y0; i1x ^= y1; } }
@@ -645,58 +403,20 @@ scan_tile_kernel(const uint8_t* __restrict__ arena, const int64_t* __restrict__ 
           if (w >= wl1) pre1 ^= tw;
         }
       }
-      }
       uint32_t nz = 0x7ff00000u;
-      const bool any_drop = CLS == CLASS_COUNTER && Mc->any_drop != 0;
       {
         const TileChunk& c0 = S.c[cc[0]]; const TileChunk& c1 = S.c[cc[1]];
 #pragma unroll
         for (int jj = 0; jj < 2; ++jj) {
           const TileChunk& ch = jj ? c1 : c0;
           const uint64_t pre = jj ? pre1 : pre0;
-          const int g = act[jj] ? (DEC ? jj * 32 + lane : warp * 8 + jj * 4 + (lane >> 3)) - ch.grp_base : 0;   // an inactive slot's chunk descriptor is not initialised
+          const int g = act[jj] ? warp * 8 + jj * 4 + (lane >> 3) - ch.grp_base : 0;   // an inactive slot's chunk descriptor is not initialised
           uint64_t* dst = reinterpret_cast<uint64_t*>(vals + (size_t)ds * L.vals_pitch + ch.row_base) + 1 + g * 8;
           const int nleft = act[jj] ? ch.nrows - 1 - g * 8 : 0;     // rows past nrows are never read as data
-          if (DEC && nleft >= 8) {                   // a full group: four 16-byte stores (dst is 16-byte aligned by construction)
-#ifdef FILO_CUSIM
-            if (reinterpret_cast<uintptr_t>(dst) & 15) { std::fprintf(stderr, "cusim: misaligned 16-byte row store (series %d chunk %d)\n", ds, cc[jj]); std::abort(); }
-#endif
-#pragma unroll
-            for (int i = 0; i < 8; i += 2) {
-              const uint64_t b0 = d[jj][i] ^ pre, b1 = d[jj][i + 1] ^ pre;
-              *reinterpret_cast<ulonglong2*>(dst + i) = make_ulonglong2(b0, b1);
-              const uint32_t e0 = ~(uint32_t)(b0 >> 32) & 0x7ff00000u, e1 = ~(uint32_t)(b1 >> 32) & 0x7ff00000u;
-              nz = e0 < nz ? e0 : nz; nz = e1 < nz ? e1 : nz;
-            }
-          } else {
 #pragma unroll
           for (int i = 0; i < 8; ++i) {
             const uint64_t b = d[jj][i] ^ pre;
             if (i < nleft) { dst[i] = b; const uint32_t e = ~(uint32_t)(b >> 32) & 0x7ff00000u; nz = e < nz ? e : nz; }
-          }
-          }
-          if (CLS == CLASS_COUNTER && FN != FN_DELTA && any_drop) {
-            // counter drops inside a drop-flagged chunk (DoubleVector.scala:330-340): row r drops when (NaN -> 0) of it is below
-            // (NaN -> 0) of row r - 1; the value before the group is the XOR prefix itself
-            if (act[jj] && CTc[ds * TILE_MAXC + cc[jj]].dropped) {
-              TileDrops& D = DRc[ds * TILE_MAXC + cc[jj]];
-              double prevv = nan0(__longlong_as_double((long long)pre));
-              uint32_t dm = 0;                 // bit i: row i of the group drops
-#pragma unroll
-              for (int i = 0; i < 8; ++i) {
-                const double cur = nan0(__longlong_as_double((long long)(d[jj][i] ^ pre)));
-                dm |= (i < nleft && cur < prevv) ? (1u << i) : 0u;
-                prevv = cur;
-              }
-              while (dm) {                     // rare: record position and amount (the value before the drop)
-                const int i = __ffs(dm) - 1; dm &= dm - 1;
-                uint64_t prevbits = pre;
-#pragma unroll
-                for (int j = 0; j < 8; ++j) if (j == i - 1) prevbits = d[jj][j] ^ pre;
-                const int at = atomicAdd(&D.n, 1);
-                if (at < TILE_MAXDROP) { D.pos[at] = 1 + g * 8 + i; D.amt[at] = nan0(__longlong_as_double((long long)prevbits)); }
-              }
-            }
           }
           if (act[jj] && g == 0) { dst[-1] = ch.first; const uint32_t e = ~(uint32_t)(ch.first >> 32) & 0x7ff00000u; nz = e < nz ? e : nz; }
         }
@@ -714,13 +434,8 @@ scan_tile_kernel(const uint8_t* __restrict__ arena, const int64_t* __restrict__ 
           const uint64_t* src = reinterpret_cast<const uint64_t*>(recbuf + ch.val_off + 8);
           uint64_t* dst = reinterpret_cast<uint64_t*>(vals + (size_t)s * L.vals_pitch + ch.row_base);
           bool nan = false;
-          const bool drp = CLS == CLASS_COUNTER && FN != FN_DELTA && CTc[s * TILE_MAXC + c].dropped;
           for (int r = tid; r < ch.nrows; r += TILE_THREADS) {
             const uint64_t b = src[r]; dst[r] = b; nan |= ((uint32_t)(b >> 32) & 0x7ff00000u) == 0x7ff00000u;
-            if (drp && r > 0) {
-              const double cur = nan0(__longlong_as_double((long long)b)), prevv = nan0(__longlong_as_double((long long)src[r - 1]));
-              if (cur < prevv) { TileDrops& D = DRc[s * TILE_MAXC + c]; const int at = atomicAdd(&D.n, 1); if (at < TILE_MAXDROP) { D.pos[at] = r; D.amt[at] = prevv; } }
-            }
           }
           if (nan) Mc->any_nan = 1;
         }
@@ -732,115 +447,17 @@ scan_tile_kernel(const uint8_t* __restrict__ arena, const int64_t* __restrict__ 
     // ------------------------------------------------------------------ windows: blocked single-chunk windows
     {
       const bool any_nan = Mc->any_nan != 0, padded = Mc->all_padded != 0;
-      if (CLS == CLASS_COUNTER) {
-        // warp w <-> series w: the unclamped single-chunk windows of each chunk, lanes over windows.  Lowest / highest sample
-        // = first / last row of the window (RateFunctions.scala:257-267); the extrapolation constants come from the producer
-        TileSeries& S = const_cast<TileSeries&>(SDc[warp]);
-        if (S.regular == 1) {
-          bool overflow = false;
-          for (int c = 0; c < S.n; ++c) overflow |= FN != FN_DELTA && CTc[warp * TILE_MAXC + c].dropped && DRc[warp * TILE_MAXC + c].n > TILE_MAXDROP;
-          if (!overflow && FN != FN_DELTA && lane < S.n && CTc[warp * TILE_MAXC + lane].dropped) {
-            // lane c: sort chunk c's drops by row and turn the amounts into running sums (reference order of additions)
-            TileDrops& D = DRc[warp * TILE_MAXC + lane];
-            const int n = D.n;
-            for (int i = 1; i < n; ++i) {
-              const int p = D.pos[i]; const double a = D.amt[i]; int j = i - 1;
-              while (j >= 0 && D.pos[j] > p) { D.pos[j + 1] = D.pos[j]; D.amt[j + 1] = D.amt[j]; --j; }
-              D.pos[j + 1] = p; D.amt[j + 1] = a;
-            }
-            double run = 0.0;
-            for (int i = 0; i < n; ++i) { run += D.amt[i]; D.amt[i] = run; }
-          }
-          __syncwarp();
-          if (overflow) {                         // more drops in one chunk than the list holds: the generic kernel takes the series
-            __syncwarp();
-            if (lane == 0) {
-              S.regular = 0; Mc->all_regular = 0;
-              if (!AGG) { const unsigned long long slot = atomicAdd(fallback_count, 1ull); fallback_list[slot] = S.sid; }
-            }
-          } else {
-            for (int c = 0; c < S.n; ++c) {
-              const TileChunk& ch = S.c[c];
-              if (ch.kA2 > ch.kB2) continue;
-              const bool hasfast = ch.kA <= ch.kB;
-              const TileCtr kc = CTc[warp * TILE_MAXC + c];
-              const TileDrops& D = DRc[warp * TILE_MAXC + c];
-              const bool drp = FN != FN_DELTA && kc.dropped;
-              const double* cv = vals + (size_t)warp * L.vals_pitch + ch.row_base;
-              double* o = otile + (size_t)warp * L.out_pitch;
-              // drops of this chunk (warp-uniform): none / one (position and amount in registers) / several (list walk)
-              const int dn = drp ? D.n : 0;
-              const int dpos0 = dn >= 1 ? D.pos[0] : 0x7fffffff;
-              const double damt0 = dn >= 1 ? D.amt[0] : 0.0;
-              for (int kk = ch.kA + lane; hasfast && kk <= ch.kB; kk += 32) {
-                const int r1 = ch.s0 + kk, r2 = ch.e0 + kk;
-                double v1 = cv[r1], v2 = cv[r2];
-                if (drp) {
-                  if (dn <= 1) { v1 = nan0(v1) + (r1 >= dpos0 ? damt0 : 0.0); v2 = nan0(v2) + (r2 >= dpos0 ? damt0 : 0.0); }
-                  else { v1 = nan0(v1) + drops_cum(D, r1); v2 = nan0(v2) + drops_cum(D, r2); }     // sorted running sums
-                }
-                const double delta = v2 - v1;
-                double ratio = kc.ratio0;
-                if (FN != FN_DELTA && delta > 0 && v1 >= 0 && !(v1 > delta * kc.skipC)) {      // zero-point clamp may apply (:84-90)
-                  const double dz = kc.sI * (v1 / delta);
-                  const double dts = dz < kc.dTS ? dz : kc.dTS;
-                  const double eTI = (kc.sI + (dts < kc.thr ? dts : kc.half)) + kc.endpart;
-                  ratio = eTI / kc.sI;
-                }
-                const double scaled = delta * ratio;
-                o[kk] = FN == FN_RATE ? __dmul_rn(div_invariant(scaled, fdiv, frcp), 1000.0) : scaled;
-              }
-              // the chunk's clamped single-chunk windows (window start before its first row or end after its last): the
-              // sample distance varies with the window, the table supplies the terms that depend on it
-              const int nlo = hasfast ? ch.kA - ch.kA2 : ch.kB2 - ch.kA2 + 1, nhi = hasfast ? ch.kB2 - ch.kB : 0;
-              for (int u = lane; u < nlo + nhi; u += 32) {
-                const int kk = u < nlo ? ch.kA2 + u : ch.kB + 1 + (u - nlo);
-                int r1 = ch.s0 + kk; if (r1 < 0) r1 = 0;
-                int r2 = ch.e0 + kk; if (r2 > ch.nrows - 1) r2 = ch.nrows - 1;
-                double res = __longlong_as_double(0x7ff8000000000000LL);
-                if (r2 > r1) {                                   // highestTime > lowestTime (RateFunctions.scala:271,284)
-                  double v1 = cv[r1], v2 = cv[r2];
-                  if (drp) { v1 = nan0(v1) + drops_cum(D, r1); v2 = nan0(v2) + drops_cum(D, r2); }
-                  const int64_t wEnd = q.start + (int64_t)kk * q.step, cws = wEnd - winDur - (q.inclusive ? 0 : 1);
-                  res = extrapolated_rate_tile<FN != FN_DELTA, FN == FN_RATE>(cws, wEnd, r2 - r1 + 1, ch.init + (int64_t)r1 * q.step, v1,
-                                                                              ch.init + (int64_t)r2 * q.step, v2, fdiv, frcp, q.step, CTAB);
-                }
-                o[kk] = res;
-              }
-            }
-            // windows outside every chunk's single-chunk interval (chunk junctions, no data): literal fold, lanes over the gaps
-            {
-              const double* sv = vals + (size_t)warp * L.vals_pitch;
-              double* o = otile + (size_t)warp * L.out_pitch;
-              int prev = -1;
-              for (int c = 0; c <= S.n; ++c) {
-                int gend = q.T;
-                if (c < S.n) { if (S.c[c].kA2 > S.c[c].kB2) continue; gend = S.c[c].kA2; }
-                for (int k = prev + 1 + lane; k < gend; k += 32) {
-                  const int64_t wEnd = q.start + (int64_t)k * q.step, wStart = wEnd - winDur;
-                  o[k] = tile_eval_counter<FN>(S, CTc + warp * TILE_MAXC, DRc + warp * TILE_MAXC, sv, q, wStart, wEnd, k, fdiv, frcp, CTAB);
-                }
-                if (c < S.n) prev = S.c[c].kB2;
-              }
-            }
-          }
-        }
-      }
-      TPROF(4)                                              // wait: barrier B (+ counter-class windows)
-      const int nitems = CLS == CLASS_COUNTER ? 0 : Mc->pref[TILE_NS];
+      TPROF(4)                                              // wait: barrier B
+      const int nitems = Mc->pref[TILE_NS];
       for (int it = tid; it < nitems; it += TILE_THREADS) {
         int s = 0;
 #pragma unroll
         for (int j = 1; j < TILE_NS; ++j) if (it >= Mc->pref[j]) s = j;
         const TileSeries& S = SDc[s];
         const int B = it - Mc->pref[s];
-        int c = 0; while (c + 1 < S.n && B >= S.c[c].blk0 + S.c[c].blk_n + S.c[c].jblk) ++c;
+        int c = 0; while (c + 1 < S.n && B >= S.c[c].blk0 + S.c[c].blk_n) ++c;
         const TileChunk& ch = S.c[c];
         const int b = B - ch.blk0;
-        if (b >= ch.blk_n) {                       // a block of the junction with the previous chunk
-          tile_junction_block<FN>(S, c, vals + (size_t)s * L.vals_pitch, otile + (size_t)s * L.out_pitch, b - ch.blk_n, any_nan, q, winDur, fdiv, frcp);
-          continue;
-        }
         const int r0 = ch.sA + b * BLK_R;
         const double* slots = vals + (size_t)s * L.vals_pitch + ch.row_base;
         double acc[BLK_R]; int cnt[BLK_R];
@@ -880,8 +497,8 @@ scan_tile_kernel(const uint8_t* __restrict__ arena, const int64_t* __restrict__ 
         }
       }
       // ---------------------------------------------------------------- windows: everything else (chunk junctions, short windows)
-      TPROF(5)                                              // windows: blocked and junction items
-      const int nrest = CLS == CLASS_COUNTER ? 0 : Mc->rpref[TILE_NS];
+      TPROF(5)                                              // windows: blocked items
+      const int nrest = Mc->rpref[TILE_NS];
       for (int it = tid; it < nrest; it += TILE_THREADS) {
         int s = 0;
 #pragma unroll
@@ -891,26 +508,21 @@ scan_tile_kernel(const uint8_t* __restrict__ arena, const int64_t* __restrict__ 
         int prev = -1; bool found = false;          // u-th window not covered by a blocked interval
         for (int c = 0; c < S.n && !found; ++c) {
           if (S.c[c].kA > S.c[c].kB) continue;
-          const int gap = S.c[c].kAj - prev - 1;
+          const int gap = S.c[c].kA - prev - 1;
           if (u < gap) found = true; else { u -= gap; prev = S.c[c].kB; }
         }
         const int k = prev + 1 + u;
-#ifdef FILO_CUSIM
-        ++cusim_rest_windows;
-#endif
         const int64_t wEnd = q.start + (int64_t)k * q.step, wStart = wEnd - winDur;
         const double* sv = vals + (size_t)s * L.vals_pitch;
-        if (CLS == CLASS_COUNTER) otile[(size_t)s * L.out_pitch + k] = tile_eval_counter<FN>(S, CTc + s * TILE_MAXC, DRc + s * TILE_MAXC, sv, q, wStart, wEnd, k, fdiv, frcp, CTAB);
-        else otile[(size_t)s * L.out_pitch + k] = any_nan ? tile_eval_window<FN, true>(S, sv, wStart, wEnd, fdiv, k)
-                                                          : tile_eval_window<FN, false>(S, sv, wStart, wEnd, fdiv, k);
+        otile[(size_t)s * L.out_pitch + k] = any_nan ? tile_eval_window<FN, true>(S, sv, wStart, wEnd, fdiv, k)
+                                                     : tile_eval_window<FN, false>(S, sv, wStart, wEnd, fdiv, k);
       }
     }
     TPROF(6)                                                // windows: literal per-window folds
     fence_async_smem();        // make this thread's writes to the output tile visible to the async proxy (bulk store below)
     bar_consumers();
     TPROF(7)                                                // wait: windows-end barrier
-    // tile flags of this tile stay valid until the producer's setup two tiles ahead, which waits for the next B barrier;
-    // a counter series whose drop list overflowed was declared irregular during the windows
+    // tile flags of this tile stay valid until the producer's setup two tiles ahead, which waits for the next B barrier
     const bool all_reg = Mc->all_regular != 0;
     // scan counters (CountingChunkInfoIterator): series this kernel answers; series / items handed to the fallback are counted there
     if (tid < ns && SDc[tid].regular == 1) { pend_rows += SDc[tid].cnt_rows; pend_bytes += SDc[tid].cnt_bytes; }

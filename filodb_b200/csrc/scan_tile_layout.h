@@ -23,15 +23,13 @@ struct TileChunk {
   uint32_t grp_off, tab_off;  // XOR vectors: byte offsets (in the staged tile) of the first group / of the u16 group table
   int32_t ngroups, grp_base;
   int32_t blk0, blk_n;
-  int32_t tlen, vlen;         // timestamp / value vector lengths
   int32_t s0, e0;             // unclamped first / last row of window k = 0 (rows advance by one per window)
   int32_t lowz, highz;        // zero rows before / after the chunk's rows (clamped windows read them as +0.0)
-  int32_t kA2, kB2;           // COUNTER: all single-chunk windows of the chunk, clamped ones included ([kA, kB] = unclamped)
-  // SUM class: the windows between the previous chunk's blocked interval and this chunk's (rows in both chunks) are folded as
-  // blocks of two partial sums when nothing else can contribute to them: jn windows from jk0 in jblk blocks; kAj = first window
-  // covered by a block of this chunk (jk0, or kA without a junction)
-  int32_t jk0, jn, jblk, kAj;
+  // unused: the descriptors keep their size, and with it tile_layout's footprint, which decides what this kernel and the v4 SUM
+  // kernel admit (filo_query)
+  int32_t spare[8];
 };
+static_assert(sizeof(TileChunk) == 128, "TileChunk");
 struct TileSeries {
   int32_t n, regular, rec_off, nblocks, nrest, ngroups, nrows, any_raw;
   int64_t sid;                // series ordinal in the table
@@ -40,45 +38,22 @@ struct TileSeries {
   TileChunk c[TILE_MAXC];
 };
 
-// COUNTER class only.  TileCtr (producer, double-buffered): per-chunk constants of the extrapolation for windows whose rows lie
-// inside the chunk and are not clamped (RateFunctions.scala:72-111 with every window-invariant subexpression evaluated once).
-struct TileCtr {
-  double dTS, thr, half, endpart, sI, ratio0, skipC;   // see scan_tile.cuh (producer) for the definitions
-  int32_t dropped, pad;
-};
-// TileDrops (consumers, per tile): counter drops of a drop-flagged chunk, found while its rows are decoded
-// (CorrectingDoubleVectorReader.corrected, DoubleVector.scala:325-342): row position and the amount added to the correction
-constexpr int TILE_MAXDROP = 8;
-// per-query table of the extrapolation terms that depend only on (numSamples - 1) = m when the samples are m steps apart
-constexpr int TILE_CTR_TABMAX = 64;
-struct TileCtrTab { double sI, thr, half, rcpSI; };      // sampledInterval, 1.1 * average interval, average / 2, RN(1 / sI)
-struct TileDrops {
-  int32_t n, pos[TILE_MAXDROP], pad[3];
-  double amt[TILE_MAXDROP];
-};
-
 struct TileMeta {                         // per-tile work-list prefixes and flags
   int32_t pref[TILE_NS + 1];              // blocked work items per series (prefix)
   int32_t rpref[TILE_NS + 1];             // other windows per series (prefix)
   int32_t any_nan, any_raw, all_regular, all_padded;
   int32_t staged, ns; int64_t i0;
-  int32_t any_drop, pad;
 };
 
 struct TileSmem {                         // byte offsets inside dynamic shared memory (all multiples of 128)
-  uint32_t rec, vals, out, desc, gtot, meta, ctr, drops, tab, total;
+  uint32_t rec, vals, out, desc, gtot, meta, total;
   uint32_t rec_cap, vals_pitch /*doubles per series*/, out_pitch /*doubles per series = T*/, desc_stride /*bytes between the two descriptor buffers*/;
-  uint32_t opts;                          // TILE_OPT_* switches (A/B measurements): set by tile_layout, cleared by the host from the environment
 };
-constexpr uint32_t TILE_OPT_JUNCTION = 1u;   // chunk-junction windows as blocks of two partial sums (FILO_TILE_JUNCTION=0 turns it off)
-constexpr uint32_t TILE_OPT_WARPDEC = 2u;    // warp w decodes series w alone (no cross-warp exchange barrier); needs the even row pitch
-                                             // and odd chunk row offsets that tile_layout / the producer set up with it (FILO_TILE_WARPDEC=1, experimental)
-FILO_HD inline TileSmem tile_layout(uint32_t max_rec_bytes, uint32_t max_rows, uint32_t T, uint32_t pad_rows, bool counter_class = false, bool warp_decode = false) {
+FILO_HD inline TileSmem tile_layout(uint32_t max_rec_bytes, uint32_t max_rows, uint32_t T, uint32_t pad_rows) {
   TileSmem L;
   L.rec_cap = align_up(TILE_NS * max_rec_bytes + 128, 128);
   L.desc_stride = align_up(TILE_NS * (uint32_t)sizeof(TileSeries), 128);
   L.vals_pitch = (max_rows + pad_rows + 2 + 1) | 1;            // odd pitch (doubles); pad_rows: zero rows for clamped windows
-  if (warp_decode) L.vals_pitch += TILE_MAXC + 1;               // even pitch + one parity row per chunk: 16-byte aligned row stores
   L.out_pitch = T;
   uint32_t o = 128;                                            // mbarrier slot
   L.rec = o; o += L.rec_cap;
@@ -87,11 +62,7 @@ FILO_HD inline TileSmem tile_layout(uint32_t max_rec_bytes, uint32_t max_rows, u
   L.desc = o; o += 2 * align_up(TILE_NS * (uint32_t)sizeof(TileSeries), 128);      // double-buffered: setup of tile t+1 overlaps tile t
   L.gtot = o; o += align_up(TILE_NS * TILE_GX_PITCH * 8 + TILE_NS * TILE_GW_PITCH * 8, 128);     // per-slot in-warp prefixes + per-warp totals (padded pitches)
   L.meta = o; o += 2 * 128;
-  L.ctr = o; L.drops = o; L.tab = o;
-  if (counter_class) { o += 2 * align_up(TILE_NS * TILE_MAXC * (uint32_t)sizeof(TileCtr), 128); L.drops = o; o += align_up(TILE_NS * TILE_MAXC * (uint32_t)sizeof(TileDrops), 128);
-                       L.tab = o; o += align_up((TILE_CTR_TABMAX + 1) * (uint32_t)sizeof(TileCtrTab), 128); }
   L.total = o;
-  L.opts = TILE_OPT_JUNCTION | (warp_decode ? TILE_OPT_WARPDEC : 0u);
   return L;
 }
 

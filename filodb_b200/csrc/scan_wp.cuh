@@ -35,6 +35,7 @@ __device__ __forceinline__ uint32_t wp_lds32(uint32_t off) { uint32_t v; asm vol
 #endif
 
 __device__ __forceinline__ int wp_vidx(int p) { return p + (p >> 3); }
+__device__ __forceinline__ double nan0(double x) { return x != x ? 0.0 : x; }
 // results are written once and not read again by the scan: streaming store
 #ifdef FILO_CUSIM
 __device__ __forceinline__ void wp_store_result(double* g, double v) { *g = v; }

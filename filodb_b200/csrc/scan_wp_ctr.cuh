@@ -1,7 +1,7 @@
 // v4 scan path, counter class: rate / increase on cumulative schemas (counter correction + Prometheus extrapolation) and delta, on the
 // per-warp pipeline of scan_wp.cuh (one warp per series, TMA-staged record, group decode into V, no CTA barriers after start-up).
 //
-// Window phase = the tile kernel's counter phase (scan_tile.cuh), warp <-> series and lanes over windows:
+// Window phase, warp <-> series and lanes over windows:
 //   * windows whose rows sit unclamped inside one chunk: the sample times move with the window, so durationToStart / End,
 //     sampledInterval and numSamples of RateFunctions.extrapolatedRate (RateFunctions.scala:72-111) are per-chunk constants of the plan;
 //     a window costs two row loads, the correction lookup, one subtraction, a test that rules out the zero-point clamp without
@@ -18,6 +18,51 @@
 
 namespace filo {
 
+// correction accumulated up to and including row r.  The list has been sorted by position and its amounts replaced by their
+// running sums in position order (start of the window phase) -- the same additions as the reference's running
+// `_correction += last` -- so the answer is the entry of the last drop at or before r.
+__device__ __forceinline__ double drops_cum(const TileDrops& D, int r) {
+  const int n = D.n < TILE_MAXDROP ? D.n : TILE_MAXDROP;
+  double cum = 0.0;
+#pragma unroll
+  for (int j = 0; j < TILE_MAXDROP; ++j) if (j < n && D.pos[j] <= r) cum = D.amt[j];
+  return cum;
+}
+
+// RateFunctions.extrapolatedRate (RateFunctions.scala:72-111), same operations in the same order; the divisions by the constants
+// 1000 and (windowEnd - windowStart) use the exact invariant-divisor sequence, and the zero-point quotient is only formed
+// when durationToZero can be below durationToStart: v1 * sI > 2 * dTS * delta  =>  sI * (v1 / delta) >= dTS
+template <bool IS_COUNTER, bool IS_RATE>
+__device__ __forceinline__ double extrapolated_rate_tile(int64_t windowStart, int64_t windowEnd, int32_t numSamples, int64_t t1, double v1,
+                                                         int64_t t2, double v2, double fdiv, double frcp, int64_t step, const TileCtrTab* tab) {
+  double durationToStart = div_invariant((double)(t1 - windowStart), 1000.0, 0.001);
+  const double durationToEnd = div_invariant((double)(windowEnd - t2), 1000.0, 0.001);
+  const int64_t si_ms = t2 - t1;
+  const int m = numSamples - 1;
+  double sampledInterval, extrapolationThreshold, half, rcpSI;
+  if (m <= TILE_CTR_TABMAX && si_ms == (int64_t)m * step) {      // samples m steps apart: the terms depend on m only (see the table)
+    const TileCtrTab e = tab[m];
+    sampledInterval = e.sI; extrapolationThreshold = e.thr; half = e.half; rcpSI = e.rcpSI;
+  } else {
+    sampledInterval = div_invariant((double)si_ms, 1000.0, 0.001);
+    const double averageDurationBetweenSamples = ddiv_rare(sampledInterval, (double)numSamples - 1.0);
+    extrapolationThreshold = averageDurationBetweenSamples * 1.1; half = averageDurationBetweenSamples / 2.0; rcpSI = 0.0;
+  }
+  const double delta = v2 - v1;
+  if (IS_COUNTER && delta > 0 && v1 >= 0) {
+    if (!(v1 * sampledInterval > 2.0 * durationToStart * delta)) {
+      const double durationToZero = sampledInterval * ddiv_rare(v1, delta);
+      if (durationToZero < durationToStart) durationToStart = durationToZero;
+    }
+  }
+  double extrapolateToInterval = sampledInterval;
+  extrapolateToInterval += (durationToStart < extrapolationThreshold) ? durationToStart : half;
+  extrapolateToInterval += (durationToEnd < extrapolationThreshold) ? durationToEnd : half;
+  const double ratio = rcpSI != 0.0 ? div_invariant(extrapolateToInterval, sampledInterval, rcpSI) : ddiv_rare(extrapolateToInterval, sampledInterval);
+  const double scaledDelta = delta * ratio;
+  return IS_RATE ? __dmul_rn(div_invariant(scaledDelta, fdiv, frcp), 1000.0) : scaledDelta;
+}
+
 __device__ __forceinline__ double wp_row(const double* V, const WpCtrChunk& ch, int r) { return V[wp_vidx(ch.rowpos + r)]; }
 // value of row r as the counter functions see it: CorrectingDoubleVectorReader.corrected for a drop-flagged chunk, raw otherwise
 __device__ __forceinline__ double wp_ctr_value(const double* V, const WpCtrChunk& ch, int r, const TileDrops& D, bool dropped) {
@@ -26,16 +71,11 @@ __device__ __forceinline__ double wp_ctr_value(const double* V, const WpCtrChunk
   return nan0(x) + drops_cum(D, r);
 }
 
-// literal per-chunk fold of the counter functions for one window: tile_eval_counter (scan_tile.cuh) over the skewed V layout
-// FILO_WP_CTR_OUTLINE: the junction fold and the clamped windows as real calls (one or two warp iterations per series go through them;
-// inlined they sit between the decode and the fast loop of every series and push the kernel's hot code out of the instruction cache)
-#if defined(FILO_WP_CTR_OUTLINE) && !defined(FILO_CUSIM)
-#define WP_CTR_RARE static __device__ __noinline__
-#else
-#define WP_CTR_RARE __device__ __forceinline__
-#endif
+// literal per-chunk fold of the counter functions for one window of a regular series: CounterChunkedRangeFunction.addChunks
+// (RangeFunction.scala:131-172), ChunkedRateFunctionBase (RateFunctions.scala:230-285), correction carry
+// (DoubleVector.scala:177-207, 375-391), over the skewed V layout
 template <int FN>
-WP_CTR_RARE double wp_eval_counter(int n, const WpCtrChunk* K, const WpChunk* CD, const TileDrops* DR, const double* V, int64_t qstep, int qinclusive,
+__device__ __forceinline__ double wp_eval_counter(int n, const WpCtrChunk* K, const WpChunk* CD, const TileDrops* DR, const double* V, int64_t qstep, int qinclusive,
                                                   int64_t wStart, int64_t wEnd, int k, double fdiv, double frcp, const TileCtrTab* tab) {
   const double NaNv = __longlong_as_double(0x7ff8000000000000LL);
   int32_t numSamples = 0; int64_t loT = INT64_MAX, hiT = 0; double loV = NaNv, hiV = NaNv;
@@ -135,9 +175,9 @@ inline void wp_bump_u16(uint16_t* p) { *p = (uint16_t)(*p + 1); }
 #else
 static __device__ __noinline__ void wp_bump_u16(uint16_t* p) { *p = (uint16_t)(*p + 1); }
 #endif
-// one clamped single-chunk window (kept out of line: one or two warp iterations per series go through it)
+// one clamped single-chunk window
 template <int FN>
-WP_CTR_RARE double wp_clamped_window(const double* V, const WpCtrChunk& ch, const TileDrops& D, bool drp, int kk, int64_t wEnd, int64_t cws, int64_t qstep,
+__device__ __forceinline__ double wp_clamped_window(const double* V, const WpCtrChunk& ch, const TileDrops& D, bool drp, int kk, int64_t wEnd, int64_t cws, int64_t qstep,
                                                    double fdiv, double frcp, const TileCtrTab* tab) {
   int r1 = ch.s0 + kk; if (r1 < 0) r1 = 0;
   int r2 = ch.e0 + kk; if (r2 > ch.nrows - 1) r2 = ch.nrows - 1;

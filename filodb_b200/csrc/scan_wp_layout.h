@@ -9,10 +9,7 @@ constexpr int WP_MAXC = 4;             // chunks in range per series on this pat
 constexpr int WP_MAXG = 64;            // NibblePack groups per series (two per lane)
 constexpr int WP_R = 8;                // windows per block
 constexpr int WP_MAX_WARPS = 16;       // warps per CTA (one CTA per SM) when O has its own region
-#ifndef FILO_WP_MAX_WARPS_ALIAS
-#define FILO_WP_MAX_WARPS_ALIAS 20
-#endif
-constexpr int WP_MAX_WARPS_ALIAS = FILO_WP_MAX_WARPS_ALIAS; // ... when O takes V's place (single-pass plans): 20 warps = 96 registers per thread (22 = 88 registers, spills)
+constexpr int WP_MAX_WARPS_ALIAS = 20; // ... when O takes V's place (single-pass plans): 20 warps = 96 registers per thread (22 = 88 registers, spills)
 
 struct WpChunk {                       // per warp, per chunk in range (shared memory)
   uint64_t first;                      // XOR vectors: bits of the first value
@@ -69,6 +66,22 @@ FILO_HD inline uint32_t wp_max_items(uint32_t max_chunks, uint32_t T, uint32_t w
 }
 
 constexpr int WP_CTR_MAX_WARPS = 20;   // counter kernel: warps per CTA at the lower register budget
+// TileCtr: per-chunk constants of the extrapolation for windows whose rows lie inside the chunk and are not clamped
+// (RateFunctions.scala:72-111 with every window-invariant subexpression evaluated once).
+struct TileCtr {
+  double dTS, thr, half, endpart, sI, ratio0, skipC;   // see the plan in scan_wp_ctr.cuh for the definitions
+  int32_t dropped, pad;
+};
+// TileDrops: counter drops of a drop-flagged chunk, found while its rows are decoded
+// (CorrectingDoubleVectorReader.corrected, DoubleVector.scala:325-342): row position and the amount added to the correction
+constexpr int TILE_MAXDROP = 8;
+// per-query table of the extrapolation terms that depend only on (numSamples - 1) = m when the samples are m steps apart
+constexpr int TILE_CTR_TABMAX = 64;
+struct TileCtrTab { double sI, thr, half, rcpSI; };      // sampledInterval, 1.1 * average interval, average / 2, RN(1 / sI)
+struct TileDrops {
+  int32_t n, pos[TILE_MAXDROP], pad[3];
+  double amt[TILE_MAXDROP];
+};
 struct WpCtrChunk {                    // per warp, per chunk in range: plan (window intervals, extrapolation constants)
   int64_t init, end_time;
   int32_t nrows, s0, e0, rowpos;
@@ -101,6 +114,15 @@ FILO_HD inline WpCtrSmem wp_ctr_layout(uint32_t max_rec_bytes, uint32_t max_rows
   L.per_warp = align_up(o, 16);
   L.tab = 0; L.warps = 0; L.agg = agg ? 1u : 0u;
   return L;
+}
+// The counter kernel takes a table only when eight of its series, staged the way the round-1 tile kernel staged counter tables
+// (tile_layout plus per-chunk extrapolation constants, drop lists and the extrapolation table), fit in `cap` bytes: the selection
+// this kernel was measured under.  Lifting the bound would move large-record counter tables from the v2 kernel to this one, a
+// speed change to be measured on its own.
+FILO_HD inline bool wp_ctr_tile_footprint_ok(uint32_t max_rec_bytes, uint32_t max_rows, uint32_t T, uint64_t cap) {
+  const uint32_t ctr = 2 * align_up(TILE_NS * TILE_MAXC * (uint32_t)sizeof(TileCtr), 128) + align_up(TILE_NS * TILE_MAXC * (uint32_t)sizeof(TileDrops), 128) +
+                       align_up((TILE_CTR_TABMAX + 1) * (uint32_t)sizeof(TileCtrTab), 128);
+  return (uint64_t)(tile_layout(max_rec_bytes, max_rows, T, 0).total + ctr) + 1024 <= cap;
 }
 
 } // namespace filo

@@ -1,6 +1,6 @@
 """Per-phase cycle profile of the tile kernel's consumer warps (profiling build, -DFILO_TILE_PROF).
     FILO_NVCC_EXTRA="-DFILO_HIST_PROF -DFILO_TILE_PROF" FILO_BUILD_OUT=scratch/libfilo_b200_prof.so python -m filodb_b200.build --force
-    python scratch/tile_prof.py [workload] [series]       # on the GPU box; workload: c2 (default), c2-counter, c5"""
+    FILO_KERNEL=v3 python scratch/tile_prof.py [workload] [series]       # on the GPU box; workload: a SUM-class one, c2 (default) or c1"""
 import ctypes as C
 import os
 import subprocess
@@ -24,7 +24,7 @@ L.filo_debug_tile_prof(out.ctypes.data, 1)
 bench.main()
 L.filo_debug_tile_prof(out.ctypes.data, 0)
 names = ["wait: tile descriptors / bytes ready", "decode: field extraction + in-warp prefix", "wait: cross-warp exchange barrier", "decode: prefixes applied, rows stored",
-         "wait: barrier B (+ counter-class windows)", "windows: blocked + junction items", "windows: literal per-window folds", "wait: windows-end barrier", "-",
+         "wait: barrier B", "windows: blocked items", "windows: literal per-window folds", "wait: windows-end barrier", "-",
          "results (fold / bulk store), loop overhead"]
 tot = float(out[:10].sum())
 print("tile kernel, consumer warps (lane 0 of each): %d warps reported, all launches of the run" % int(out[15]))

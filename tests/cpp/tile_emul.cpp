@@ -87,27 +87,17 @@ struct Launch {
   int64_t* flist; unsigned long long* fcount; unsigned long long* counters; int* derr;
   const int32_t* order; const int64_t* item_begin; int64_t n_items; int agg_op; double* pval; uint32_t* pcnt;
 };
-template <int CLS, int FN, bool AGG> static void run_kernel(const Launch& A) {
-  if (A.L.opts & filo::TILE_OPT_WARPDEC) {      // as launch_tile_fn picks it
-    cusim::launch(dim3((unsigned)A.grid), dim3(filo::TILE_LAUNCH_THREADS), [&] {
-      filo::scan_tile_kernel<CLS, FN, AGG, 1>(A.arena, A.rec_off, A.S, A.q, A.out, A.L, A.flist, A.fcount, A.counters, A.derr, A.order, A.item_begin, A.n_items, A.agg_op, A.pval, A.pcnt);
-    });
-    return;
-  }
+template <int FN, bool AGG> static void run_kernel(const Launch& A) {
   cusim::launch(dim3((unsigned)A.grid), dim3(filo::TILE_LAUNCH_THREADS), [&] {
-    filo::scan_tile_kernel<CLS, FN, AGG, 0>(A.arena, A.rec_off, A.S, A.q, A.out, A.L, A.flist, A.fcount, A.counters, A.derr, A.order, A.item_begin, A.n_items, A.agg_op, A.pval, A.pcnt);
+    filo::scan_tile_kernel<FN, AGG>(A.arena, A.rec_off, A.S, A.q, A.out, A.L, A.flist, A.fcount, A.counters, A.derr, A.order, A.item_begin, A.n_items, A.agg_op, A.pval, A.pcnt);
   });
 }
 template <bool AGG> static void dispatch(const Launch& A) {          // the instantiations launch_tile_any makes (scan_kernels.cu)
   const int fn = A.q.fn;
-  if (filo::fn_class_of(fn, A.q.cumulative) == filo::CLASS_COUNTER) {
-    if (fn == filo::FN_RATE) run_kernel<filo::CLASS_COUNTER, filo::FN_RATE, AGG>(A);
-    else if (fn == filo::FN_INCREASE) run_kernel<filo::CLASS_COUNTER, filo::FN_INCREASE, AGG>(A);
-    else run_kernel<filo::CLASS_COUNTER, filo::FN_DELTA, AGG>(A);
-  } else if (fn == filo::FN_RATE) run_kernel<filo::CLASS_SUM, filo::FN_RATE, AGG>(A);
-  else if (fn == filo::FN_AVG) run_kernel<filo::CLASS_SUM, filo::FN_AVG, AGG>(A);
-  else if (fn == filo::FN_COUNT) run_kernel<filo::CLASS_SUM, filo::FN_COUNT, AGG>(A);
-  else run_kernel<filo::CLASS_SUM, filo::FN_SUM, AGG>(A);
+  if (fn == filo::FN_RATE) run_kernel<filo::FN_RATE, AGG>(A);
+  else if (fn == filo::FN_AVG) run_kernel<filo::FN_AVG, AGG>(A);
+  else if (fn == filo::FN_COUNT) run_kernel<filo::FN_COUNT, AGG>(A);
+  else run_kernel<filo::FN_SUM, AGG>(A);
 }
 // the v2 warp-per-series kernel (every function / encoding; also the fallback pass over the series the tile kernel declined)
 struct V2Shape { uint32_t max_rec; int max_rows, max_chunks; bool any_nonconst_ts, any_drop; };
@@ -164,55 +154,50 @@ int main(int argc, char** argv) {
   std::mt19937_64 rng(4242);
   long checked = 0; int cases = 0;
   struct Cfg { int kind = 0; bool xor_enc = true; int fn = 0; std::vector<int> chunks; int nan_ppm = 0, reset_every = 0; int64_t window = 300000; int nser = 1; int inclusive = 1;
-               int64_t start_off = 0, end_off = 0; int agg_op = 0; int grid = 1; int jitter = 0; bool integral = false; bool v2_only = false; bool no_junction = false; bool warp_decode = false; bool wp = false; bool hetero = false; int long_col = 0; double p0 = 0, p1 = 0; };
+               int64_t start_off = 0, end_off = 0; int agg_op = 0; int grid = 1; int jitter = 0; bool integral = false; bool v2_only = false; bool wp = false; bool hetero = false; int long_col = 0; double p0 = 0, p1 = 0; };
   std::vector<Cfg> all_ext;
   const std::vector<Cfg> cfgs = {
     {0, true, filo::FN_RATE, {400, 80}, 200000, 0, 300000, 11, 1, 0, 0, 0, 2},           // C2: gauge, delta-temporality rate (CLASS_SUM), NaN stale markers
     {0, true, filo::FN_SUM, {150, 90}, 0, 0, 300000, 37, 1, -90000, 45000, 0, 2},        // several tiles per CTA, a partial last tile, windows before / after the data
-    {0, true, filo::FN_SUM, {150, 90}, 0, 0, 300000, 13, 1, -90000, 45000, 0, 2, 0, false, false, true},   // the same with junction blocks switched off (FILO_TILE_JUNCTION=0)
+    {0, true, filo::FN_SUM, {150, 90}, 0, 0, 300000, 13, 1, -90000, 45000, 0, 2},        // the same, two tiles
     {0, false, filo::FN_AVG, {200, 40}, 100000, 0, 120000, 5, 0, 0, 0, 0, 1},             // raw f64 vectors, exclusive range start
     {0, true, filo::FN_COUNT, {60, 60, 60, 60}, 300000, 0, 600000, 9, 1, 30000, 0, 0, 3}, // four chunks, long windows over several chunk junctions
     {0, true, filo::FN_RATE, {100, 50, 50, 50, 50}, 0, 0, 300000, 10, 1, 0, 0, 0, 2},     // five chunks: declined (fallback list)
     {0, true, filo::FN_AVG, {100, 100, 100}, 30000, 0, 300000, 24, 1, 0, 0, 0, 2},        // two junctions per series, NaN rows in some tiles only
     {0, true, filo::FN_COUNT, {90, 70, 50, 30}, 0, 0, 240000, 16, 0, 15000, 0, 0, 2},     // three junctions, exclusive range start, a chunk barely longer than the window
-    {0, false, filo::FN_SUM, {64, 200}, 0, 0, 420000, 9, 1, 0, 0, 0, 1},                  // raw vectors, 29-window junction (two blocks)
-    {1, true, filo::FN_RATE, {400, 80}, 0, 0, 300000, 10, 1, 0, 0, 0, 2},                 // counters: extrapolated rate (CLASS_COUNTER)
-    {1, true, filo::FN_INCREASE, {120, 120, 60}, 0, 41, 60000, 19, 1, -30000, 30000, 0, 2}, // resets: drop-flagged chunks, corrections across chunks
-    {1, false, filo::FN_DELTA, {200, 100}, 0, 0, 300000, 6, 0, 0, 0, 0, 1},               // delta over raw vectors
-    // the per-warp decode variant of the tile kernel (FILO_TILE_WARPDEC=1): C2 shape with NaN markers, three chunks, raw + XOR mixes
-    {0, true, filo::FN_RATE, {400, 80}, 200000, 0, 300000, 19, 1, 0, 0, 0, 2, 0, false, false, false, true},
-    {0, true, filo::FN_AVG, {100, 100, 100}, 30000, 0, 300000, 24, 1, -30000, 30000, 0, 2, 0, false, false, false, true},
-    {0, true, filo::FN_SUM, {33, 150, 7, 90}, 0, 0, 240000, 11, 0, 0, 0, 0, 3, 0, false, false, false, true},
-    {1, true, filo::FN_RATE, {400, 80}, 0, 61, 300000, 13, 1, 0, 0, 0, 2, 0, false, false, false, true},            // ... counters with resets
-    {1, true, filo::FN_INCREASE, {120, 120, 60}, 0, 41, 60000, 12, 1, -30000, 30000, filo::AGG_SUM, 2, 0, false, false, false, true},   // ... fused
+    {0, false, filo::FN_SUM, {64, 200}, 0, 0, 420000, 9, 1, 0, 0, 0, 1},                  // raw vectors, a 29-window junction
+    {0, true, filo::FN_RATE, {400, 80}, 200000, 0, 300000, 19, 1, 0, 0, 0, 2},           // C2 shape with NaN markers, three tiles
+    {0, true, filo::FN_AVG, {100, 100, 100}, 30000, 0, 300000, 24, 1, -30000, 30000, 0, 2},  // three chunks, windows before / after the data
+    {0, true, filo::FN_SUM, {33, 150, 7, 90}, 0, 0, 240000, 11, 0, 0, 0, 0, 3},           // a 7-row chunk inside the windows, raw + XOR mixes
     // the v4 warp-pipeline kernel (scan_wp.cuh) for the SUM class, declines chained to the v2 kernel
-    {0, true, filo::FN_RATE, {400, 80}, 200000, 0, 300000, 23, 1, 0, 0, 0, 2, 0, false, false, false, false, true},                 // C2 shape, NaN stale markers (declined)
-    {0, true, filo::FN_SUM, {150, 90}, 0, 0, 300000, 37, 1, -90000, 45000, 0, 2, 0, false, false, false, false, true},              // windows before / after the data
-    {0, false, filo::FN_AVG, {200, 40}, 0, 0, 180000, 9, 0, 0, 0, 0, 1, 0, false, false, false, false, true},                       // raw f64, exclusive range start
-    {0, true, filo::FN_COUNT, {60, 60, 60, 60}, 0, 0, 600000, 9, 1, 30000, 0, 0, 3, 0, false, false, false, false, true},           // four chunks, windows over three chunks (declined)
-    {0, true, filo::FN_AVG, {100, 100, 100}, 0, 0, 300000, 24, 1, 0, 0, 0, 2, 0, false, false, false, false, true},                 // two junctions
-    {0, true, filo::FN_COUNT, {90, 70, 50, 30}, 0, 0, 240000, 16, 0, 15000, 0, 0, 2, 0, false, false, false, false, true},          // three junctions, exclusive start
-    {0, false, filo::FN_SUM, {64, 200}, 0, 0, 420000, 9, 1, 0, 0, 0, 1, 0, false, false, false, false, true},
-    {0, true, filo::FN_RATE, {100, 50, 50, 50, 50}, 0, 0, 300000, 10, 1, 0, 0, 0, 2, 0, false, false, false, false, true},          // five chunks: declined
-    {0, true, filo::FN_SUM, {33, 150, 7, 90}, 0, 0, 240000, 11, 0, 0, 0, 0, 3, 0, false, false, false, false, true},                // a 7-row chunk inside the windows
-    {0, false, filo::FN_RATE, {500, 400}, 0, 0, 300000, 7, 1, 0, 0, 0, 1, 0, false, false, false, false, true},                      // more than 64 blocks per series: second pass
-    {0, true, filo::FN_SUM, {150, 90}, 0, 0, 300000, 29, 1, -90000, 45000, 0, 2, 0, false, false, false, false, true, true},          // chunk shapes differ from series to series: the plan memo is invalidated
-    {0, false, filo::FN_AVG, {200, 100}, 0, 0, 180000, 21, 0, 0, 0, 0, 1, 0, false, false, false, false, true, true},
+    {0, true, filo::FN_RATE, {400, 80}, 200000, 0, 300000, 23, 1, 0, 0, 0, 2, 0, false, false, true},                 // C2 shape, NaN stale markers (declined)
+    {0, true, filo::FN_SUM, {150, 90}, 0, 0, 300000, 37, 1, -90000, 45000, 0, 2, 0, false, false, true},              // windows before / after the data
+    {0, false, filo::FN_AVG, {200, 40}, 0, 0, 180000, 9, 0, 0, 0, 0, 1, 0, false, false, true},                       // raw f64, exclusive range start
+    {0, true, filo::FN_COUNT, {60, 60, 60, 60}, 0, 0, 600000, 9, 1, 30000, 0, 0, 3, 0, false, false, true},           // four chunks, windows over three chunks (declined)
+    {0, true, filo::FN_AVG, {100, 100, 100}, 0, 0, 300000, 24, 1, 0, 0, 0, 2, 0, false, false, true},                 // two junctions
+    {0, true, filo::FN_COUNT, {90, 70, 50, 30}, 0, 0, 240000, 16, 0, 15000, 0, 0, 2, 0, false, false, true},          // three junctions, exclusive start
+    {0, false, filo::FN_SUM, {64, 200}, 0, 0, 420000, 9, 1, 0, 0, 0, 1, 0, false, false, true},
+    {0, true, filo::FN_RATE, {100, 50, 50, 50, 50}, 0, 0, 300000, 10, 1, 0, 0, 0, 2, 0, false, false, true},          // five chunks: declined
+    {0, true, filo::FN_SUM, {33, 150, 7, 90}, 0, 0, 240000, 11, 0, 0, 0, 0, 3, 0, false, false, true},                // a 7-row chunk inside the windows
+    {0, false, filo::FN_RATE, {500, 400}, 0, 0, 300000, 7, 1, 0, 0, 0, 1, 0, false, false, true},                      // more than 64 blocks per series: second pass
+    {0, true, filo::FN_SUM, {150, 90}, 0, 0, 300000, 29, 1, -90000, 45000, 0, 2, 0, false, false, true, true},          // chunk shapes differ from series to series: the plan memo is invalidated
+    {0, false, filo::FN_AVG, {200, 100}, 0, 0, 180000, 21, 0, 0, 0, 0, 1, 0, false, false, true, true},
     // the v4 counter-class kernel (scan_wp_ctr.cuh): per-series and fused, resets (drop lists), raw vectors, delta
-    {1, true, filo::FN_RATE, {400, 80}, 0, 0, 300000, 10, 1, 0, 0, 0, 2, 0, false, false, false, false, true},
-    {1, true, filo::FN_INCREASE, {120, 120, 60}, 0, 41, 60000, 19, 1, -30000, 30000, 0, 2, 0, false, false, false, false, true},
-    {1, false, filo::FN_DELTA, {200, 100}, 0, 0, 300000, 6, 0, 0, 0, 0, 1, 0, false, false, false, false, true},
-    {1, true, filo::FN_RATE, {400, 80}, 200000, 61, 300000, 13, 1, 0, 0, 0, 2, 0, false, false, false, false, true},                  // NaN markers + resets
-    {1, true, filo::FN_RATE, {150, 90}, 0, 7, 300000, 21, 1, 0, 0, 0, 2, 0, false, false, false, false, true, true},                   // frequent resets (drop list overflow -> declined), shapes differ
-    {1, true, filo::FN_INCREASE, {120, 120, 60}, 0, 41, 60000, 12, 1, -30000, 30000, filo::AGG_SUM, 2, 0, false, false, false, false, true},   // fused
-    {1, true, filo::FN_RATE, {240, 240}, 0, 97, 300000, 17, 1, 0, 0, filo::AGG_MAX, 2, 0, false, false, false, false, true},
-    {1, true, filo::FN_RATE, {100, 50, 50, 50, 50}, 0, 0, 300000, 12, 1, 0, 0, filo::AGG_SUM, 2, 0, false, false, false, false, true},  // fused, every item declined
+    {1, true, filo::FN_RATE, {400, 80}, 0, 0, 300000, 10, 1, 0, 0, 0, 2, 0, false, false, true},
+    {1, true, filo::FN_INCREASE, {120, 120, 60}, 0, 41, 60000, 19, 1, -30000, 30000, 0, 2, 0, false, false, true},
+    {1, false, filo::FN_DELTA, {200, 100}, 0, 0, 300000, 6, 0, 0, 0, 0, 1, 0, false, false, true},
+    {1, true, filo::FN_RATE, {400, 80}, 200000, 61, 300000, 13, 1, 0, 0, 0, 2, 0, false, false, true},                  // NaN markers + resets
+    {1, true, filo::FN_RATE, {400, 80}, 0, 61, 300000, 13, 1, 0, 0, 0, 2, 0, false, false, true},                       // resets without NaN markers
+    {1, true, filo::FN_RATE, {150, 90}, 0, 7, 300000, 21, 1, 0, 0, 0, 2, 0, false, false, true, true},                   // frequent resets (drop list overflow -> declined), shapes differ
+    {1, true, filo::FN_INCREASE, {120, 120, 60}, 0, 41, 60000, 12, 1, -30000, 30000, filo::AGG_SUM, 2, 0, false, false, true},   // fused
+    {1, true, filo::FN_RATE, {240, 240}, 0, 97, 300000, 17, 1, 0, 0, filo::AGG_MAX, 2, 0, false, false, true},
+    {1, true, filo::FN_RATE, {100, 50, 50, 50, 50}, 0, 0, 300000, 12, 1, 0, 0, filo::AGG_SUM, 2, 0, false, false, true},  // fused, every item declined
     // irregular scrapes (DDV timestamps with residuals) on the v4 counter kernel: searched row ranges, literal fold per window
-    {1, true, filo::FN_RATE, {400, 80}, 0, 61, 300000, 9, 1, 0, 0, 0, 2, 2000, false, false, false, false, true},
-    {1, true, filo::FN_INCREASE, {120, 120, 60}, 50000, 41, 60000, 11, 0, -30000, 30000, 0, 2, 4000, false, false, false, false, true},
-    {1, false, filo::FN_DELTA, {200, 100}, 0, 0, 300000, 6, 1, 0, 0, 0, 1, 700, false, false, false, false, true},
-    {1, true, filo::FN_INCREASE, {150, 150}, 0, 45, 60000, 14, 1, 0, 0, filo::AGG_SUM, 2, 2000, false, false, false, false, true},      // fused (BASELINE C3 shape)
-    {1, true, filo::FN_RATE, {240, 240}, 100000, 97, 300000, 13, 1, 15000, 0, filo::AGG_MAX, 2, 3000, false, false, false, false, true, true},
+    {1, true, filo::FN_RATE, {400, 80}, 0, 61, 300000, 9, 1, 0, 0, 0, 2, 2000, false, false, true},
+    {1, true, filo::FN_INCREASE, {120, 120, 60}, 50000, 41, 60000, 11, 0, -30000, 30000, 0, 2, 4000, false, false, true},
+    {1, false, filo::FN_DELTA, {200, 100}, 0, 0, 300000, 6, 1, 0, 0, 0, 1, 700, false, false, true},
+    {1, true, filo::FN_INCREASE, {150, 150}, 0, 45, 60000, 14, 1, 0, 0, filo::AGG_SUM, 2, 2000, false, false, true},      // fused (BASELINE C3 shape)
+    {1, true, filo::FN_RATE, {240, 240}, 100000, 97, 300000, 13, 1, 15000, 0, filo::AGG_MAX, 2, 3000, false, false, true, true},
     // the v2 warp-per-series kernel on its own: every function class, irregular scrapes (DDV timestamps), integral values (DDV longs)
     {0, true, filo::FN_MIN, {150, 90}, 100000, 0, 300000, 9, 1, -30000, 15000, 0, 2, 0, false, true},
     {0, false, filo::FN_MAX, {64, 64, 64, 64, 64}, 0, 0, 200000, 7, 0, 0, 0, 0, 1, 0, false, true},
@@ -224,7 +209,6 @@ int main(int argc, char** argv) {
     // tile kernel + fallback pass: irregular scrapes make the tile kernel decline every series
     {0, true, filo::FN_RATE, {200, 100}, 0, 0, 300000, 10, 1, 0, 0, 0, 2, 4000, false, false},
     {0, true, filo::FN_RATE, {400, 80}, 100000, 0, 300000, 26, 1, 0, 0, filo::AGG_SUM, 2},   // fused sum: items of 5 series in shuffled order
-    {1, true, filo::FN_RATE, {240, 240}, 0, 97, 300000, 17, 1, 0, 0, filo::AGG_MAX, 2},      // fused max over counters with resets
   };
   // the remaining chunked range functions and the Long-column variants: window by window on the v2 kernel (eval_window_ext)
   {
@@ -277,9 +261,8 @@ int main(int argc, char** argv) {
       c.jitter = fr() % 5 == 0 ? 300 + (int)(fr() % 5000) : 0;
       c.integral = fr() % 6 == 0; if (c.integral) c.xor_enc = false;
       c.v2_only = fr() % 4 == 0;
-      c.no_junction = fr() % 8 == 0;
-      c.warp_decode = fr() % 3 == 0;
-      c.wp = fr() % 2 == 0;
+      fr(); fr();                      // two unused draws: a seed keeps drawing the shapes it always drew
+      c.wp = fr() % 2 == 0;            // SUM class: v4 or tile kernel (the counter class always takes the v4 counter kernel)
       c.hetero = fr() % 3 == 0;
       if (c.v2_only) { const int fns[] = {filo::FN_MIN, filo::FN_MAX, filo::FN_LAST, filo::FN_TIMESTAMP, c.fn, c.fn}; c.fn = fns[fr() % 6]; c.agg_op = 0; }
       all.push_back(c);
@@ -311,11 +294,9 @@ int main(int argc, char** argv) {
     if (q.end < q.start) q.end = q.start;
     q.T = (int)((q.end - q.start) / q.step) + 1;
     q.fn = c.fn; q.cumulative = c.kind == 1; q.inclusive = c.inclusive; q.long_values = c.long_col ? 1 : 0; q.p0 = c.p0; q.p1 = c.p1;
-    if (c.agg_op && q.T > filo::TILE_AGG_ACC * filo::TILE_THREADS) c.agg_op = 0;      // the fused tile path serves T <= 512 (filo_query picks the other kernels beyond)
-    const bool ctr = filo::fn_class_of(q.fn, q.cumulative, q.long_values) == filo::CLASS_COUNTER;
+    if (c.agg_op && q.T > filo::TILE_AGG_ACC * filo::TILE_THREADS) c.agg_op = 0;      // the fused tile / v4 counter paths serve T <= 512 (filo_query picks the v2 kernel beyond)
     const uint32_t wrows = (uint32_t)(q.window / q.step) + 1;
-    filo::TileSmem L = filo::tile_layout(max_rec, (uint32_t)rows, (uint32_t)q.T, ctr ? 0u : 2 * wrows + 16, ctr, c.warp_decode);
-    if (c.no_junction) L.opts &= ~filo::TILE_OPT_JUNCTION;
+    const filo::TileSmem L = filo::tile_layout(max_rec, (uint32_t)rows, (uint32_t)q.T, 2 * wrows + 16);
     if (L.total > sizeof(filo::smem)) { std::printf("FAIL: layout %u bytes\n", L.total); return 1; }
     // oracle, per series
     std::vector<double> ref((size_t)c.nser * q.T); std::vector<int64_t> oracle_rows((size_t)c.nser, 0);
@@ -351,7 +332,7 @@ int main(int argc, char** argv) {
         if (derr[0]) { std::printf("FAIL cfg %zu: device error %d (wp kernel)\n", ci, derr[0]); return 1; }
         g_wp_declined += (long)fcount; g_wp_series += c.nser;
         if (fcount) run_v2(A, sh, flist.data(), &fcount);
-      } else if (tile_ok && c.wp && cls == filo::CLASS_COUNTER) {
+      } else if (tile_ok && cls == filo::CLASS_COUNTER) {
         filo::WpCtrSmem W = filo::wp_ctr_layout(max_rec, (uint32_t)rows, (uint32_t)c.chunks.size(), (uint32_t)q.T, false, c.jitter != 0);
         W.warps = 3; W.tab = W.per_warp * W.warps;
         if ((size_t)W.tab + 4096 > sizeof(filo::smem)) { std::printf("FAIL: wp ctr layout %u bytes per warp\n", W.per_warp); return 1; }
@@ -384,8 +365,7 @@ int main(int argc, char** argv) {
       }
       if ((int64_t)counters[0] != exp_rows) { std::printf("FAIL cfg %zu: samples_scanned %llu vs %lld\n", ci, counters[0], (long long)exp_rows); return 1; }
       if (tile_ok && c.chunks.size() > (size_t)filo::TILE_MAXC && fcount != (unsigned long long)c.nser) { std::printf("FAIL cfg %zu: series with too many chunks were not declined\n", ci); return 1; }
-      if (!quiet) std::printf("cfg %zu ok: %d series (%llu to the fallback list), T=%d; junction blocks %ld, literal windows %ld\n", ci, c.nser, fcount, q.T, filo::cusim_junction_blocks, filo::cusim_rest_windows);
-      filo::cusim_junction_blocks = filo::cusim_rest_windows = 0;
+      if (!quiet) std::printf("cfg %zu ok: %d series (%llu to the fallback list), T=%d\n", ci, c.nser, fcount, q.T);
     } else {
       // items of <= 5 series in a shuffled order (what build_groups produces for one group)
       std::vector<int32_t> order((size_t)c.nser); for (int s = 0; s < c.nser; ++s) order[(size_t)s] = s;
@@ -394,7 +374,7 @@ int main(int argc, char** argv) {
       const int64_t n_items = (int64_t)item_begin.size() - 1;
       std::vector<double> pval((size_t)n_items * q.T, -777.0); std::vector<uint32_t> pcnt((size_t)n_items * q.T, 12345u);
       A.order = order.data(); A.item_begin = item_begin.data(); A.n_items = n_items; A.agg_op = c.agg_op; A.pval = pval.data(); A.pcnt = pcnt.data(); A.out = nullptr;
-      if (c.wp && filo::fn_class_of(q.fn, q.cumulative) == filo::CLASS_COUNTER) {
+      if (filo::fn_class_of(q.fn, q.cumulative) == filo::CLASS_COUNTER) {
         filo::WpCtrSmem W = filo::wp_ctr_layout(max_rec, (uint32_t)rows, (uint32_t)c.chunks.size(), (uint32_t)q.T, true, c.jitter != 0);
         W.warps = 3; W.tab = W.per_warp * W.warps;
         if ((size_t)W.tab + 4096 > sizeof(filo::smem)) { std::printf("FAIL: wp ctr layout %u bytes per warp\n", W.per_warp); return 1; }
