@@ -394,6 +394,13 @@ extern "C" int filo_debug_tile_prof(unsigned long long* out16, int reset) {
   return (int)e;
 }
 #endif
+#ifdef FILO_WP_PROF
+extern "C" int filo_debug_wp_prof(unsigned long long* out16, int reset) {
+  cudaError_t e = cudaMemcpyFromSymbol(out16, g_wp_prof, sizeof(unsigned long long) * 16);
+  if (e == cudaSuccess && reset) { unsigned long long z[16] = {}; e = cudaMemcpyToSymbol(g_wp_prof, z, sizeof z); }
+  return (int)e;
+}
+#endif
 // ---------------------------------------------------------------------------------------------------------------
 // host-callable launchers
 // ---------------------------------------------------------------------------------------------------------------

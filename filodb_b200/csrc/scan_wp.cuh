@@ -2,12 +2,14 @@
 //
 // Each warp runs its own three-buffer pipeline in shared memory:
 //   R  the series' record (ChunkSetInfo entries + BinaryVectors verbatim), filled by ONE cp.async.bulk (TMA 1-D) per series that is
-//      issued as soon as the previous record has been decoded, i.e. it is in flight during the previous series' window phase;
+//      issued as soon as the previous record is no longer read (its fields extracted, raw f64 vectors copied), i.e. it is in flight
+//      during the rest of the previous series' decode and its window phase;
 //   V  the decoded rows, laid out per chunk with zero rows in between so that clamped windows read +0.0 instead of testing bounds
-//      (x + 0.0 is exact for an accumulator that started at +0.0), skewed by one pad slot per 8 rows: both the 8-byte row stores of the
+//      (x + 0.0 == x for every sum of non-zero values and +0.0 rows), skewed by one pad slot per 8 rows: both the 8-byte row stores of the
 //      group decode (lane stride 8 rows) and the 8-byte row loads of the window blocks (lane stride 8 windows) then walk the banks with
 //      an odd stride of 9 words -- conflict-free;
-//   O  the series' T results, leaving with one cp.async.bulk store that overlaps the next series' decode.
+//   O  the series' T results, in V's place when the plan allows it; they leave as lane-consecutive streaming stores (256 contiguous
+//      bytes per store instruction) once every window is finished.
 // Phases of a series (all 32 lanes, only __syncwarp between them):
 //   setup    lane c = chunk c: header parse, regularity checks, window plan (touch interval, block list, row positions).  The plan
 //            depends on (init, nrows, endTime) of the chunks only, so it is reused while consecutive series share those (memo);
@@ -32,6 +34,23 @@ __device__ __forceinline__ uint32_t wp_lds32(uint32_t off) { uint32_t v; std::me
 #else
 __device__ __forceinline__ uint32_t wp_soff(const void* p) { return smem_u32(p); }
 __device__ __forceinline__ uint32_t wp_lds32(uint32_t off) { uint32_t v; asm volatile("ld.shared.u32 %0, [%1];" : "=r"(v) : "r"(off)); return v; }
+#endif
+
+// Per-phase cycle counters of scan_wp_sum_kernel for profiling builds (-DFILO_WP_PROF; scratch/wp_prof.py): every lane reads the
+// SM clock at the phase boundaries of a series, lane 0 adds its sums to g_wp_prof (slots 0 .. 9: phases, 10 .. 13: event counts,
+// 15: warps).  32-bit sums (a warp's share of one launch is far below 2^32 cycles) keep the register cost low.  Compiled out of the
+// product build.
+#if defined(FILO_WP_PROF) && !defined(FILO_CUSIM)
+__device__ unsigned long long g_wp_prof[16];
+#define WPROF_DECL uint32_t wpp_t0 = (uint32_t)clock(), wpp_acc[14] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
+#define WPROF(i) { const uint32_t wpp_t1 = (uint32_t)clock(); wpp_acc[i] += wpp_t1 - wpp_t0; wpp_t0 = wpp_t1; }
+#define WPROF_COUNT(i) { ++wpp_acc[i]; }
+#define WPROF_FLUSH if (lane == 0) { for (int wpp_i = 0; wpp_i < 14; ++wpp_i) atomicAdd(&g_wp_prof[wpp_i], (unsigned long long)wpp_acc[wpp_i]); atomicAdd(&g_wp_prof[15], 1ull); }
+#else
+#define WPROF_DECL
+#define WPROF(i)
+#define WPROF_COUNT(i)
+#define WPROF_FLUSH
 #endif
 
 __device__ __forceinline__ int wp_vidx(int p) { return p + (p >> 3); }
@@ -77,14 +96,15 @@ __device__ __forceinline__ void wp_block_tail(const double* __restrict__ pa, con
 }
 
 // two blocks per lane: a[w] / b[w] = sum of rows w .. w + Wr (in row order, starting from +0.0) of the block at pa / pb.  Wr >= 8.
+// A window's sum starts at its first row instead of at +0.0 + that row: the same bits, because every row the windows read is either a
+// decoded value (finite, normal, non-zero, or the series is declined before its windows) or a +0.0 zero row, and +0.0 + x == x for both.
 __device__ __forceinline__ void wp_block_pair(const double* __restrict__ pa, const double* __restrict__ pb, int Wr, double a[WP_R], double b[WP_R]) {
 #pragma unroll
-  for (int w = 0; w < 8; ++w) { a[w] = 0.0; b[w] = 0.0; }
-#pragma unroll
-  for (int t = 0; t < 8; ++t) {                        // group 0: row t feeds windows 0 .. t
+  for (int t = 0; t < 8; ++t) {                        // group 0: row t opens window t and feeds windows 0 .. t - 1
     const double va = pa[t], vb = pb[t];
 #pragma unroll
-    for (int w = 0; w <= t; ++w) { a[w] += va; b[w] += vb; }
+    for (int w = 0; w < t; ++w) { a[w] += va; b[w] += vb; }
+    a[t] = va; b[t] = vb;
   }
   const int q = Wr >> 3;
   pa += 9; pb += 9;
@@ -191,9 +211,12 @@ __device__ __forceinline__ WpParsed wp_parse(const uint8_t* R, const QueryParams
 // 10 and 9 different, i.e. 2^-511 <= |v| < 2^513 (finite, normal, not zero).  DROPS (counter class): counter drops inside drop-flagged
 // chunks (DoubleVector.scala:330-340) are recorded as (row, amount) in DR[chunk]; row r drops when (NaN -> 0) of it is below
 // (NaN -> 0) of row r - 1, the amount is the value before the drop.
-template <bool DROPS>
+// r_done() is called, by the whole warp, as soon as R is not read any more: right after the field extraction, or after the raw copy when
+// a chunk has raw f64 values (any_raw is the same on every lane).
+struct WpNoop { __device__ __forceinline__ void operator()() const {} };
+template <bool DROPS, typename RDone = WpNoop>
 __device__ __forceinline__ uint32_t wp_decode(const uint8_t* R, double* V, const WpChunk* CD, uint64_t* xtab, const int dd_dst[2], const int dd_inf[2],
-                                              int n, bool any_raw, int lane, TileDrops* DR) {
+                                              int n, bool any_raw, int lane, TileDrops* DR, RDone r_done = RDone()) {
   uint32_t okbits = 0xffffffffu;
   uint64_t d[2][8];
 #pragma unroll
@@ -222,6 +245,7 @@ __device__ __forceinline__ uint32_t wp_decode(const uint8_t* R, double* V, const
       d[jj][i] = x;
     }
   }
+  if (!any_raw) r_done();
   // exclusive XOR scan of the group totals over the 64 slots
   uint64_t i0x = d[0][7], i1x = d[1][7];
 #pragma unroll
@@ -285,6 +309,7 @@ __device__ __forceinline__ uint32_t wp_decode(const uint8_t* R, double* V, const
       }
     }
   }
+  if (any_raw) r_done();
   return okbits;
 }
 
@@ -356,15 +381,22 @@ scan_wp_sum_kernel(const uint8_t* __restrict__ arena, const int64_t* __restrict_
   int64_t cur_off = 0; uint32_t cur_sz = 0;
   if (s < n_series) { cur_off = rec_off[s]; cur_sz = (uint32_t)(rec_off[s + 1] - cur_off); }
   if (s < n_series && cur_sz <= L.rec_cap && lane == 0) issue(cur_off, cur_sz);
+  WPROF_DECL
 
   for (; s < n_series; s += nwarps) {
     const int64_t sn = s + nwarps;
-    int64_t nxt_off = 0; uint32_t nxt_sz = 0;
-    if (sn < n_series) { nxt_off = rec_off[sn]; nxt_sz = (uint32_t)(rec_off[sn + 1] - nxt_off); }
+    // the next record's offsets: loaded here, their difference taken after the parse, so that the loads' latency passes behind it
+    int64_t nxt_off = 0; uint32_t nxt_end = 0;                 // (the size needs the low word of the end only)
+    if (sn < n_series) { nxt_off = rec_off[sn]; nxt_end = (uint32_t)rec_off[sn + 1]; }
     const bool staged = cur_sz <= L.rec_cap;
+    WPROF_COUNT(10)
+    WPROF(9)                                               // loop head (+ the declined series' exits)
     if (staged) { mbar_wait(bar, parity); parity ^= 1; }
+    WPROF(0)                                               // wait: record
     // ------------------------------------------------------------------------------------------------ setup (lane c = chunk c)
     const WpParsed P = wp_parse<true>(R, q, staged, lane);
+    const uint32_t nxt_sz = nxt_end - (uint32_t)nxt_off;
+    WPROF(1)                                               // parse
     bool regular = P.regular;
     const bool have = P.have; const int n = P.n, c = lane;
     const int64_t init = P.init, end_time = P.end_time;
@@ -375,6 +407,7 @@ scan_wp_sum_kernel(const uint8_t* __restrict__ arena, const int64_t* __restrict_
     const bool same_all = __all_sync(FULL, samec);
     const bool same = m_ok && n == m_n && same_all;
     if (regular && !same) {
+      WPROF_COUNT(11)
       m_init = init; m_end = end_time; m_nrows = nrows; m_n = n; m_wire = vwire; m_ok = false;
       int64_t s0 = 0, e0 = 0;
       if (have) { s0 = sd.ceil_div(S0 - init); e0 = sd.floor_div(E0 - init); }
@@ -480,8 +513,10 @@ scan_wp_sum_kernel(const uint8_t* __restrict__ arena, const int64_t* __restrict_
         m_ok = true;
       }
     }
+    WPROF(2)                                               // memo check (+ window plan on a miss)
     if (!regular) {
       // declined: the v2 kernel answers this series
+      WPROF_COUNT(12)
       if (lane == 0) { const unsigned long long slot = atomicAdd(fallback_count, 1ull); fallback_list[slot] = s; }
       __syncwarp();
       if (sn < n_series && nxt_sz <= L.rec_cap && lane == 0) issue(nxt_off, nxt_sz);
@@ -503,13 +538,19 @@ scan_wp_sum_kernel(const uint8_t* __restrict__ arena, const int64_t* __restrict_
 #pragma unroll
     for (int o = 1; o < WP_MAXC; o <<= 1) { cnt_rows += __shfl_xor_sync(FULL, cnt_rows, o); cnt_bytes += __shfl_xor_sync(FULL, cnt_bytes, o); }
     __syncwarp();
+    WPROF(3)                                               // per-series descriptors, scan counters
     // ------------------------------------------------------------------------------------------------ decode
-    const uint32_t okbits = wp_decode<false>(R, V, CD, xtab, dd_dst, dd_inf, n, any_raw, lane, nullptr);
+    // R is dead once its fields are extracted: the next record's copy starts there and runs behind the rest of the decode and the
+    // window phase (every lane has read its fields when the copy is issued)
+    auto rec_done = [&]() {
+      __syncwarp();
+      if (sn < n_series && nxt_sz <= L.rec_cap && lane == 0) issue(nxt_off, nxt_sz);
+    };
+    const uint32_t okbits = wp_decode<false>(R, V, CD, xtab, dd_dst, dd_inf, n, any_raw, lane, nullptr, rec_done);
     const bool vals_ok = __all_sync(FULL, (okbits >> 30) & 1u);
     __syncwarp();
-    // R is dead: fetch the next record behind the window phase
-    if (sn < n_series && nxt_sz <= L.rec_cap && lane == 0) issue(nxt_off, nxt_sz);
     cur_off = nxt_off; cur_sz = nxt_sz;
+    WPROF(4)                                               // decode (+ the next record's copy issued)
     // zero rows (the last group of an XOR chunk decoded up to 7 rows past the chunk; results of the previous series when O is in V's place)
     if (gz_all) {
 #pragma unroll
@@ -522,8 +563,10 @@ scan_wp_sum_kernel(const uint8_t* __restrict__ arena, const int64_t* __restrict_
         for (int pz = g0 + lane; pz < g1; pz += 32) V[wp_vidx(pz)] = 0.0;
       }
     }
+    WPROF(5)                                               // zero rows
     if (!vals_ok) {
       // NaN / Inf / zero / denormal / very large or small values: the literal kernel answers (it needs the NaN-aware sums)
+      WPROF_COUNT(13)
       if (lane == 0) { const unsigned long long slot = atomicAdd(fallback_count, 1ull); fallback_list[slot] = s; }
       __syncwarp();
       continue;
@@ -580,6 +623,7 @@ scan_wp_sum_kernel(const uint8_t* __restrict__ arena, const int64_t* __restrict_
         }
       }
       __syncwarp();
+      WPROF(6)                                             // window blocks
       // raw blocks: a window with rows from two chunks is (0 + partial of the earlier chunk) + partial of the later one
       // (AggrOverTimeFunctions.scala:560-571); own windows that sit in a raw block are finished here as well
       for (int ci = 0; ci < n; ++ci) {
@@ -618,6 +662,7 @@ scan_wp_sum_kernel(const uint8_t* __restrict__ arena, const int64_t* __restrict_
     }
     // ------------------------------------------------------------------------------------------------ result row
     __syncwarp();
+    WPROF(7)                                               // junction fix-up, gaps
     {
       // lane-consecutive windows: 256 contiguous bytes per store instruction; O index of window lane + 32 m = oidx(lane) + 36 m
       double* gp = out + (size_t)s * q.T + lane;
@@ -630,7 +675,10 @@ scan_wp_sum_kernel(const uint8_t* __restrict__ arena, const int64_t* __restrict_
       for (; iters > 0; --iters, gp += 32, sp += 36) wp_store_result(gp, *sp);
     }
     __syncwarp();
+    WPROF(8)                                               // result row
   }
+  WPROF(9)
+  WPROF_FLUSH
   if (lane == 0) {
     if (rows_scanned | bytes_scanned) { atomicAdd(&d_counters[0], (unsigned long long)rows_scanned); atomicAdd(&d_counters[1], (unsigned long long)bytes_scanned); }
   }
