@@ -9,7 +9,8 @@ LIB_PATH = os.environ.get("FILO_LIB_PATH") or os.path.join(_HERE, "libfilo_b200.
 FN_LAST, FN_RATE, FN_INCREASE, FN_DELTA, FN_SUM_OVER_TIME, FN_AVG_OVER_TIME, FN_COUNT_OVER_TIME, \
     FN_MIN_OVER_TIME, FN_MAX_OVER_TIME, FN_TIMESTAMP, FN_STDDEV_OVER_TIME, FN_STDVAR_OVER_TIME, FN_CHANGES, FN_QUANTILE_OVER_TIME, \
     FN_ZSCORE, FN_HOLT_WINTERS, FN_PREDICT_LINEAR, FN_MAD_OVER_TIME, FN_PRESENT_OVER_TIME = range(19)
-AGG_NONE, AGG_SUM, AGG_AVG, AGG_MIN, AGG_MAX, AGG_COUNT, AGG_TOPK, AGG_BOTTOMK = range(8)
+AGG_NONE, AGG_SUM, AGG_AVG, AGG_MIN, AGG_MAX, AGG_COUNT, AGG_TOPK, AGG_BOTTOMK, AGG_STDDEV, AGG_STDVAR, AGG_GROUP = range(11)
+AGG_MOMENTS = (AGG_STDDEV, AGG_STDVAR)          # partial form: values [2, G, T] = (Σv, Σv²)
 SCHEMA_CUMULATIVE = 1
 SCHEMA_LONG_VALUES = 2
 Q_PARTIAL = 1
@@ -318,24 +319,26 @@ class Context:
         self._check(lib().filo_synth_table(self.h, C.byref(spec), C.byref(h)))
         return Table(self, h)
 
-    def out_shapes(self, table, start, step, end, aggr, k):
+    def out_shapes(self, table, start, step, end, aggr, k, flags=0):
         ti = table.info()
         T = num_windows(start, step if step > 0 else 1, end)
         if aggr == AGG_NONE:
             return (ti.n_series, T), None
         if aggr in (AGG_TOPK, AGG_BOTTOMK):
             return (ti.n_groups, T, k), (ti.n_groups, T, k)
+        if aggr in AGG_MOMENTS and flags & Q_PARTIAL:
+            return (2, ti.n_groups, T), (ti.n_groups, T)
         return (ti.n_groups, T), (ti.n_groups, T)
 
     def query(self, table, fn, start, step, end, window, aggr=AGG_NONE, k=0, flags=0):
         """PeriodicSamplesMapper(+AggregateMapReduce) -> host numpy arrays (values[, aux])."""
-        vs, as_ = self.out_shapes(table, start, step, end, aggr, k)
+        vs, as_ = self.out_shapes(table, start, step, end, aggr, k, flags)
         out = np.zeros(vs, np.float64)
         aux = np.zeros(as_, np.int64) if as_ is not None else None
         st = Stats()
         self._check(lib().filo_query(self.h, table.h, fn, start, step, end, window, aggr, k, flags, _p(out), _p(aux), C.byref(st)))
         self.last_stats = st.as_dict()
-        if aggr in (AGG_AVG, AGG_TOPK, AGG_BOTTOMK) or (flags & Q_PARTIAL and aggr != AGG_NONE):
+        if aggr in (AGG_AVG, AGG_TOPK, AGG_BOTTOMK, AGG_STDDEV, AGG_STDVAR, AGG_GROUP) or (flags & Q_PARTIAL and aggr != AGG_NONE):
             return out, aux
         return out
 

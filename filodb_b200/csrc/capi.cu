@@ -826,7 +826,7 @@ static int32_t query_device_impl(filo_ctx* ctx, const filo_table* t, int32_t fn,
     if (!(ctx->fn_args[0] >= 0 && ctx->fn_args[0] <= 1)) return fail(ctx, FILO_ERR_INVALID_ARG, "Sf should be in between 0 and 1");
     if (!(ctx->fn_args[1] >= 0 && ctx->fn_args[1] <= 1)) return fail(ctx, FILO_ERR_INVALID_ARG, "tf should be in between 0 and 1");
   }
-  if (agg < FILO_AGG_NONE || agg > FILO_AGG_BOTTOMK) return fail(ctx, FILO_ERR_INVALID_ARG, "unknown aggregation operator");
+  if (agg < FILO_AGG_NONE || agg > FILO_AGG_GROUP) return fail(ctx, FILO_ERR_INVALID_ARG, "unknown aggregation operator");
   // PeriodicSamplesMapper.scala:45-49, 67-68
   if (start > end) return fail(ctx, FILO_ERR_INVALID_ARG, "start should be <= end");
   if (!(start == end || step > 0)) return fail(ctx, FILO_ERR_INVALID_ARG, "step should be > 0 for range query");
@@ -848,6 +848,10 @@ static int32_t query_device_impl(filo_ctx* ctx, const filo_table* t, int32_t fn,
   q.long_values = long_values ? 1 : 0; q.p0 = ctx->fn_args[0]; q.p1 = ctx->fn_args[1];
   const bool need_corr = (fn == FILO_FN_RATE || fn == FILO_FN_INCREASE) && q.cumulative;
   const bool fused = (agg != FILO_AGG_NONE && agg != FILO_AGG_TOPK && agg != FILO_AGG_BOTTOMK);
+  // stddev / stdvar: the scan kernels fold (Σv, Σv², n) in their SUM mode plus a Σv² row; group folds the count partial.  Only
+  // the merge / presentation sees the operator itself.
+  const bool moments = agg_moments(agg);
+  const int scan_op = moments ? AGG_SUM : agg == FILO_AGG_GROUP ? AGG_COUNT : agg;
 
   Temp tmp(s);
   int* d_err = nullptr; unsigned long long* d_counters = nullptr;
@@ -861,7 +865,7 @@ static int32_t query_device_impl(filo_ctx* ctx, const filo_table* t, int32_t fn,
   //      v1 (generic, global-memory record reads, optional global scratch) takes everything else.  The v4 kernels and the tile
   //      kernel run in front of v2 where they apply.  FILO_KERNEL=v1 forces v1, v2 forces v2, v3 keeps the SUM class on the tile
   //      kernel (the other classes on v2).
-  const uint32_t acc_bytes = fused ? align_up((uint32_t)q.T * 12u, 128) : 0;
+  const uint32_t acc_bytes = fused ? align_up((uint32_t)q.T * (moments ? 20u : 12u), 128) : 0;
   const bool need_corr2 = need_corr && t->any_drop;
   uint32_t scratch2 = align_up((uint32_t)t->max_chunks * (uint32_t)CHUNK_DESC_BYTES, 16) +
                       ((uint32_t)t->max_rows + (uint32_t)t->max_chunks * 8u) * 8u * (1u + (t->any_nonconst_ts ? 1u : 0u) + (need_corr2 ? 1u : 0u));
@@ -922,7 +926,7 @@ static int32_t query_device_impl(filo_ctx* ctx, const filo_table* t, int32_t fn,
   bool use_wp_ctr = false;
   if (use_v2 && force != "v2" && force != "v3" && fn_cls == CLASS_COUNTER && t->n_series > 0 && t->max_chunks > 0 &&
       (!fused || q.T <= TILE_AGG_ACC * TILE_THREADS) && wp_ctr_tile_footprint_ok(t->max_rec_bytes, (uint32_t)t->max_rows, (uint32_t)q.T, smem_cap)) {
-    WC = wp_ctr_layout(t->max_rec_bytes, (uint32_t)t->max_rows, (uint32_t)t->max_chunks, (uint32_t)q.T, fused, t->any_nonconst_ts);
+    WC = wp_ctr_layout(t->max_rec_bytes, (uint32_t)t->max_rows, (uint32_t)t->max_chunks, (uint32_t)q.T, fused, t->any_nonconst_ts, moments);
     // the irregular-timestamp instantiation is built for <= 16 warps
     const size_t w = std::min<size_t>((smem_cap - sizeof(TileCtrTab) * (TILE_CTR_TABMAX + 1) - 64) / WC.per_warp, WC.tsr != 0 ? 16 : WP_CTR_MAX_WARPS);
     WC.warps = (uint32_t)w; WC.tab = (uint32_t)(WC.per_warp * w);
@@ -972,7 +976,7 @@ static int32_t query_device_impl(filo_ctx* ctx, const filo_table* t, int32_t fn,
     launches += 1;
   } else {
     double* pval = nullptr; uint32_t* pcnt = nullptr;
-    CUDA_TRY(ctx, tmp.alloc((void**)&pval, (size_t)t->n_items * q.T * 8));
+    CUDA_TRY(ctx, tmp.alloc((void**)&pval, (size_t)t->n_items * q.T * 8 * (moments ? 2 : 1)));      // moments: [2][n_items][T]
     CUDA_TRY(ctx, tmp.alloc((void**)&pcnt, (size_t)t->n_items * q.T * 4));
     const int32_t* order = t->grouped ? t->d_order : nullptr;
     if ((use_tile && q.T <= TILE_AGG_ACC * TILE_THREADS) || use_wp_ctr) {
@@ -984,18 +988,19 @@ static int32_t query_device_impl(filo_ctx* ctx, const filo_table* t, int32_t fn,
       ScanLaunch LT = L;
       if (use_wp_ctr) {
         LT.grid = (int)std::max<int64_t>(1, std::min<int64_t>((t->n_items + WC.warps - 1) / WC.warps, (int64_t)ctx->sm_count));
-        CUDA_TRY(ctx, launch_scan_wp_ctr_agg(LT, WC, order, t->d_item_begin, t->n_items, agg, pval, pcnt, d_list, d_cnt));
+        CUDA_TRY(ctx, launch_scan_wp_ctr_agg(LT, WC, order, t->d_item_begin, t->n_items, scan_op, pval, pcnt, d_list, d_cnt, moments));
       } else {
         const int ctas_per_sm = ((size_t)TL.total + 1024) * 2 <= (size_t)228 * 1024 ? 2 : 1;
         LT.grid = (int)std::max<int64_t>(1, std::min<int64_t>(t->n_items, (int64_t)ctx->sm_count * ctas_per_sm));
-        CUDA_TRY(ctx, launch_scan_tile_agg(LT, TL, order, t->d_item_begin, t->n_items, agg, pval, pcnt, d_list, d_cnt));
+        CUDA_TRY(ctx, launch_scan_tile_agg(LT, TL, order, t->d_item_begin, t->n_items, scan_op, pval, pcnt, d_list, d_cnt, moments));
       }
       ScanLaunch LF = L; LF.list = d_list; LF.list_count = d_cnt;
-      CUDA_TRY(ctx, launch_scan_agg_v2(LF, order, t->d_item_begin, t->n_items, agg, pval, pcnt, acc_bytes, rec_cap_used));
+      CUDA_TRY(ctx, launch_scan_agg_v2(LF, order, t->d_item_begin, t->n_items, scan_op, pval, pcnt, acc_bytes, rec_cap_used, moments));
       launches += 1;
     } else {
-      CUDA_TRY(ctx, use_v2 ? launch_scan_agg_v2(L, order, t->d_item_begin, t->n_items, agg, pval, pcnt, acc_bytes, rec_cap_used)
-                           : launch_scan_agg(L, order, t->d_item_begin, t->n_items, agg, pval, pcnt, acc_bytes));
+      // (the v1 kernel reads the moments mode from the operator itself)
+      CUDA_TRY(ctx, use_v2 ? launch_scan_agg_v2(L, order, t->d_item_begin, t->n_items, scan_op, pval, pcnt, acc_bytes, rec_cap_used, moments)
+                           : launch_scan_agg(L, order, t->d_item_begin, t->n_items, moments ? agg : scan_op, pval, pcnt, acc_bytes));
     }
     CUDA_TRY(ctx, launch_merge_partials(pval, pcnt, t->d_gis, t->n_groups, q.T, agg, (flags & FILO_Q_PARTIAL) ? 1 : 0,
                                         (double*)d_out_values, (int64_t*)d_out_aux, s));
@@ -1043,7 +1048,7 @@ static int32_t filo_query_impl(filo_ctx* ctx, const filo_table* t, int32_t fn, i
   size_t nvals, naux = 0;
   if (agg == FILO_AGG_NONE) nvals = (size_t)t->n_series * T;
   else if (agg == FILO_AGG_TOPK || agg == FILO_AGG_BOTTOMK) { if (k <= 0 || k > FILO_MAX_TOPK) return fail(ctx, FILO_ERR_INVALID_ARG, "topk/bottomk k must be in [1, 32]"); nvals = naux = (size_t)t->n_groups * T * k; }
-  else { nvals = (size_t)t->n_groups * T; naux = nvals; }
+  else { naux = (size_t)t->n_groups * T; nvals = naux * ((flags & FILO_Q_PARTIAL) && agg_moments(agg) ? 2 : 1); }      // partial moments: Σv, Σv² blocks
   cudaStream_t s = ctx->stream;
   double* d_vals = nullptr; int64_t* d_aux = nullptr;
   CUDA_TRY(ctx, cudaMallocAsync((void**)&d_vals, std::max<size_t>(nvals, 1) * 8, s));

@@ -11,7 +11,13 @@ constexpr int FAST_WARPS = 4;          // v2 kernels
 constexpr int FAST_MIN_CTAS = 4;       // register budget of the v2 kernels: 4 CTAs x 128 threads per SM (<= 128 regs/thread)
 constexpr int CHUNK_DESC_BYTES = 144;  // sizeof(ChunkDesc), scan_device.cuh
 constexpr int FILO_MAX_TOPK = 32;
-enum { AGG_NONE = 0, AGG_SUM = 1, AGG_AVG = 2, AGG_MIN = 3, AGG_MAX = 4, AGG_COUNT = 5, AGG_TOPK = 6, AGG_BOTTOMK = 7 };
+enum { AGG_NONE = 0, AGG_SUM = 1, AGG_AVG = 2, AGG_MIN = 3, AGG_MAX = 4, AGG_COUNT = 5, AGG_TOPK = 6, AGG_BOTTOMK = 7,
+       AGG_STDDEV = 8, AGG_STDVAR = 9, AGG_GROUP = 10 };
+// stddev / stdvar fold the moments (Σv, Σv², n) of an (item, window): the scan kernels run their SUM mode plus a second partial block
+__host__ __device__ inline bool agg_moments(int agg_op) { return agg_op == AGG_STDDEV || agg_op == AGG_STDVAR; }
+// a variable of the moments instantiation of a kernel only: the other instantiations declare nothing (their code stays as it was)
+template <bool ON, typename T> struct MomOnly { T v; };
+template <typename T> struct MomOnly<false, T> {};
 
 struct QueryParams;
 
@@ -33,12 +39,13 @@ cudaError_t launch_scan_series(const ScanLaunch& L, double* out);
 cudaError_t launch_scan_agg(const ScanLaunch& L, const int32_t* order, const int64_t* item_begin, int64_t n_items, int agg_op,
                             double* pval, uint32_t* pcnt, uint32_t acc_bytes);
 cudaError_t launch_scan_series_v2(const ScanLaunch& L, double* out, uint32_t rec_cap);
+// moments: pval holds [2][n_items][T] (Σv, then Σv²); agg_op is then AGG_SUM
 cudaError_t launch_scan_agg_v2(const ScanLaunch& L, const int32_t* order, const int64_t* item_begin, int64_t n_items, int agg_op,
-                               double* pval, uint32_t* pcnt, uint32_t acc_bytes, uint32_t rec_cap);
+                               double* pval, uint32_t* pcnt, uint32_t acc_bytes, uint32_t rec_cap, bool moments = false);
 size_t v2_smem_per_warp(uint32_t rec_cap, uint32_t scratch_bytes, uint32_t acc_bytes);
 cudaError_t launch_scan_tile(const ScanLaunch& L, double* out, const TileSmem& T, int64_t* fallback_list, unsigned long long* fallback_count);
 cudaError_t launch_scan_tile_agg(const ScanLaunch& L, const TileSmem& T, const int32_t* order, const int64_t* item_begin, int64_t n_items, int agg_op,
-                                 double* pval, uint32_t* pcnt, int64_t* fallback_list, unsigned long long* fallback_count);
+                                 double* pval, uint32_t* pcnt, int64_t* fallback_list, unsigned long long* fallback_count, bool moments = false);
 cudaError_t launch_merge_partials(const double* pval, const uint32_t* pcnt, const int64_t* gis, int n_groups, int T, int agg_op,
                                   int partial_out, double* out_val, int64_t* out_cnt, cudaStream_t s);
 cudaError_t launch_present(int agg_op, int64_t n, const double* vals, const int64_t* cnts, double* out, cudaStream_t s);
@@ -49,7 +56,7 @@ cudaError_t launch_scan_wp(const ScanLaunch& L, double* out, const WpSmem& W, in
 struct WpCtrSmem;
 cudaError_t launch_scan_wp_ctr(const ScanLaunch& L, double* out, const WpCtrSmem& W, int64_t* fallback_list, unsigned long long* fallback_count);
 cudaError_t launch_scan_wp_ctr_agg(const ScanLaunch& L, const WpCtrSmem& W, const int32_t* order, const int64_t* item_begin, int64_t n_items, int agg_op,
-                                   double* pval, uint32_t* pcnt, int64_t* fallback_list, unsigned long long* fallback_count);
+                                   double* pval, uint32_t* pcnt, int64_t* fallback_list, unsigned long long* fallback_count, bool moments = false);
 size_t hist_smem_bytes(int max_rows, int nb, int T, bool agg, uint32_t max_rec);
 cudaError_t launch_hist_scan(const ScanLaunch& L, int nb, int max_rows, uint32_t max_rec, const int32_t* order, const int64_t* item_begin, int64_t n_items, int agg,
                              double* out, double* pval, uint8_t* pany);

@@ -88,6 +88,7 @@ scan_series_kernel(const uint8_t* __restrict__ arena, const int64_t* __restrict_
 // Work item = run of <= SEG consecutive series (in group-sorted order) of ONE group.  The warp folds the item's series
 // into per-window accumulators (shared memory, or global scratch when T is large) and writes one partial row:
 //   pval[item*T + k] = Σ non-NaN (SUM/AVG/COUNT) | min | max ;  pcnt[item*T + k] = number of non-NaN inputs
+//   STDDEV/STDVAR (moments): pval[item*T + k] = Σv, pval[(n_items + item)*T + k] = Σv² (accumulators [T] Σv, [T] Σv², [T] counts)
 // A second kernel folds the partial rows of each group in item order (deterministic, atomics-free).
 // ---------------------------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(SCAN_WARPS * 32)
@@ -101,8 +102,10 @@ scan_agg_kernel(const uint8_t* __restrict__ arena, const int64_t* __restrict__ r
   const int64_t gw = (int64_t)blockIdx.x * SCAN_WARPS + warp, nw = (int64_t)gridDim.x * SCAN_WARPS;
   const uint32_t per_warp = scratch_bytes + acc_bytes;
   uint8_t* base = use_smem ? smem + (size_t)warp * per_warp : gscratch + (size_t)gw * per_warp;
+  const bool mom = agg_moments(agg_op);
   double* acc = reinterpret_cast<double*>(base);
-  uint32_t* cnt = reinterpret_cast<uint32_t*>(base + (size_t)q.T * 8);
+  double* acc2 = acc + q.T;                                  // moments only
+  uint32_t* cnt = reinterpret_cast<uint32_t*>(base + (size_t)q.T * (mom ? 16 : 8));
   uint8_t* scratch = base + acc_bytes;
   const int fn = q.fn;
   const bool need_corrected = ((fn == FN_RATE || fn == FN_INCREASE) && q.cumulative);
@@ -110,7 +113,7 @@ scan_agg_kernel(const uint8_t* __restrict__ arena, const int64_t* __restrict__ r
                      : agg_op == AGG_MAX ? __longlong_as_double(0xfff0000000000000LL) : 0.0;
   int64_t rows = 0, bytes = 0;
   for (int64_t it = gw; it < n_items; it += nw) {
-    for (int k = lane; k < q.T; k += 32) { acc[k] = ident; cnt[k] = 0; }
+    for (int k = lane; k < q.T; k += 32) { acc[k] = ident; cnt[k] = 0; if (mom) acc2[k] = 0.0; }
     const int64_t b = item_begin[it], e = item_begin[it + 1];
     for (int64_t pos = b; pos < e; ++pos) {
       const int64_t i = order ? order[pos] : pos;
@@ -128,12 +131,14 @@ scan_agg_kernel(const uint8_t* __restrict__ arena, const int64_t* __restrict__ r
           else if (agg_op == AGG_COUNT) a = a;             // count only
           else a += v;
           acc[k] = a; cnt[k] += 1;
+          if (mom) acc2[k] += v * v;
         }
       }
       __syncwarp();
     }
     double* pv = pval + (size_t)it * q.T; uint32_t* pc = pcnt + (size_t)it * q.T;
     for (int k = lane; k < q.T; k += 32) { pv[k] = acc[k]; pc[k] = cnt[k]; }
+    if (mom) { double* pv2 = pval + (size_t)(n_items + it) * q.T; for (int k = lane; k < q.T; k += 32) pv2[k] = acc2[k]; }
     __syncwarp();
   }
   if (lane == 0 && (rows | bytes)) { atomicAdd(&d_counters[0], (unsigned long long)rows); atomicAdd(&d_counters[1], (unsigned long long)bytes); }
@@ -142,6 +147,29 @@ scan_agg_kernel(const uint8_t* __restrict__ arena, const int64_t* __restrict__ r
 // Fold the partial rows of each group (items [gis[g], gis[g+1])) in item order.  Block = (32 windows) x (8 item lanes);
 // thread (kk, j) folds items j, j+8, ... sequentially, then the 8 lanes are folded in fixed order -> deterministic.
 // partial_out: values/counts in mergeable form; otherwise presented (NaN when count == 0; Σ/n for AVG; n for COUNT).
+// EXT = MERGE_MOMENTS (STDDEV/STDVAR): the Σv² rows follow the Σv rows (pval + n_items * T, n_items = gis[n_groups]) and are folded
+// by the same tree; their mergeable form is [2][n_groups][T].  EXT = MERGE_GROUP: the count partial, presented as 1.0 / NaN.
+// RowAggregator.present of one merged cell: s = Σ (or min / max), s2 = Σv² (moments), c = non-NaN inputs
+__device__ __forceinline__ double present_cell(int agg_op, double s, double s2, int64_t c) {
+  const double NaNv = __longlong_as_double(0x7ff8000000000000LL);
+  if (c == 0) return NaNv;
+  if (agg_op == AGG_AVG) return s / (double)c;
+  if (agg_op == AGG_COUNT) return (double)c;
+  if (agg_op == AGG_GROUP) return 1.0;                      // GroupRowAggregator.scala:23-29
+  if (agg_moments(agg_op)) {
+    // sumSquare/count - mean^2 (StdvarRowAggregator.scala:52-72); stddev = Math.pow(stdvar, 0.5) (StddevRowAggregator.scala:51):
+    // sqrt for x >= +0, NaN below zero, with pow(-0.0, 0.5) = +0.0 and pow(-Inf, 0.5) = +Inf
+    const double m = s / (double)c;
+    const double var = s2 / (double)c - m * m;
+    if (agg_op == AGG_STDVAR) return var;
+    if (var < 0.0) return var == -__longlong_as_double(0x7ff0000000000000LL) ? __longlong_as_double(0x7ff0000000000000LL) : NaNv;
+    return var == 0.0 ? 0.0 : sqrt(var);
+  }
+  return s;
+}
+
+enum { MERGE_PLAIN = 0, MERGE_MOMENTS = 1, MERGE_GROUP = 2 };
+template <int EXT = MERGE_PLAIN>
 __global__ void __launch_bounds__(256)
 merge_partials_kernel(const double* __restrict__ pval, const uint32_t* __restrict__ pcnt, const int64_t* __restrict__ gis,
                       int n_groups, int T, int agg_op, int partial_out, double* __restrict__ out_val, int64_t* __restrict__ out_cnt) {
@@ -153,16 +181,21 @@ merge_partials_kernel(const double* __restrict__ pval, const uint32_t* __restric
   const double ident = agg_op == AGG_MIN ? __longlong_as_double(0x7ff0000000000000LL)
                      : agg_op == AGG_MAX ? __longlong_as_double(0xfff0000000000000LL) : 0.0;
   double a = ident; unsigned long long c = 0;
+  constexpr bool MOM = EXT == MERGE_MOMENTS;
+  MomOnly<MOM, double> a2;
+  if constexpr (MOM) a2.v = 0.0;
   if (k < T) {
     for (int64_t it = gis[g] + j; it < gis[g + 1]; it += 8) {
       const double v = pval[(size_t)it * T + k]; const uint32_t n = pcnt[(size_t)it * T + k];
       if (n) {
         if (agg_op == AGG_MIN) a = v < a ? v : a; else if (agg_op == AGG_MAX) a = v > a ? v : a; else a += v;
+        if constexpr (MOM) a2.v += pval[(size_t)(gis[n_groups] + it) * T + k];
         c += n;
       }
     }
   }
   sv[j][kk] = a; sc[j][kk] = c;
+  if constexpr (MOM) { __shared__ double sv2[8][33]; sv2[j][kk] = a2.v; __syncthreads(); if (j == 0 && k < T) for (int jj = 1; jj < 8; ++jj) if (sc[jj][kk]) a2.v += sv2[jj][kk]; }
   __syncthreads();
   if (j == 0 && k < T) {
     for (int jj = 1; jj < 8; ++jj) {
@@ -170,7 +203,12 @@ merge_partials_kernel(const double* __restrict__ pval, const uint32_t* __restric
       if (n) { if (agg_op == AGG_MIN) a = v < a ? v : a; else if (agg_op == AGG_MAX) a = v > a ? v : a; else a += v; c += n; }
     }
     const size_t o = (size_t)g * T + k;
-    if (partial_out) { out_val[o] = a; if (out_cnt) out_cnt[o] = (int64_t)c; }
+    if constexpr (EXT != MERGE_PLAIN) {
+      double s2 = 0.0;
+      if constexpr (MOM) s2 = a2.v;
+      if (partial_out) { out_val[o] = a; if constexpr (MOM) out_val[(size_t)n_groups * T + o] = s2; if (out_cnt) out_cnt[o] = (int64_t)c; }
+      else { out_val[o] = present_cell(agg_op, a, s2, (int64_t)c); if (out_cnt) out_cnt[o] = (int64_t)c; }
+    } else if (partial_out) { out_val[o] = a; if (out_cnt) out_cnt[o] = (int64_t)c; }
     else {
       const double NaNv = __longlong_as_double(0x7ff8000000000000LL);
       double r;
@@ -183,17 +221,11 @@ merge_partials_kernel(const double* __restrict__ pval, const uint32_t* __restric
   }
 }
 
-// present after a cross-GPU merge of partials
+// present after a cross-GPU merge of partials (STDDEV/STDVAR: the Σv² block follows the n cells of Σv)
 __global__ void present_kernel(int agg_op, int64_t n, const double* __restrict__ vals, const int64_t* __restrict__ cnts, double* __restrict__ out) {
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
-  const int64_t c = cnts[i]; const double v = vals[i];
-  double r;
-  if (c == 0) r = __longlong_as_double(0x7ff8000000000000LL);
-  else if (agg_op == AGG_AVG) r = v / (double)c;
-  else if (agg_op == AGG_COUNT) r = (double)c;
-  else r = v;
-  out[i] = r;
+  out[i] = present_cell(agg_op, vals[i], agg_moments(agg_op) ? vals[n + i] : 0.0, cnts[i]);
 }
 
 // topk / bottomk over per-series results (TopBottomKRowAggregator.scala:84-95): one thread per (group, window) scans the
@@ -315,7 +347,8 @@ scan_series_kernel_v2(const uint8_t* __restrict__ arena, const int64_t* __restri
   if (lane == 0 && (rows | bytes)) { atomicAdd(&d_counters[0], (unsigned long long)rows); atomicAdd(&d_counters[1], (unsigned long long)bytes); }
 }
 
-template <int CLS>
+// MOM: stddev / stdvar moments (agg_op = AGG_SUM): a [T] Σv² row, written to pval + n_items * T
+template <int CLS, bool MOM = false>
 __global__ void __launch_bounds__(FAST_WARPS * 32, FAST_MIN_CTAS)
 scan_agg_kernel_v2(const uint8_t* __restrict__ arena, const int64_t* __restrict__ rec_off, const int32_t* __restrict__ order,
                    const int64_t* __restrict__ item_begin, int64_t n_items,
@@ -323,6 +356,8 @@ scan_agg_kernel_v2(const uint8_t* __restrict__ arena, const int64_t* __restrict_
                    uint32_t rec_cap, uint32_t scratch_bytes, uint32_t acc_bytes,
                    unsigned long long* d_counters, int* d_err,
                    const int64_t* __restrict__ list, const unsigned long long* __restrict__ list_count) {
+  MomOnly<MOM, double*> pval2;
+  if constexpr (MOM) pval2.v = pval + (size_t)n_items * q.T;            // (all items of the query, before the list narrows them)
   if (list) n_items = (int64_t)*list_count;              // fallback pass of the tile kernel: only the listed items
   extern __shared__ __align__(128) uint8_t smem[];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -332,7 +367,9 @@ scan_agg_kernel_v2(const uint8_t* __restrict__ arena, const int64_t* __restrict_
   WarpStage st{reinterpret_cast<uint64_t*>(base), base + WARP_HDR_BYTES, rec_cap, 0, false, arena, rec_off};
   double* stage = reinterpret_cast<double*>(base + WARP_HDR_BYTES + rec_cap);
   double* acc = reinterpret_cast<double*>(base + WARP_HDR_BYTES + rec_cap + STAGE_BYTES);
-  uint32_t* cnt = reinterpret_cast<uint32_t*>(base + WARP_HDR_BYTES + rec_cap + STAGE_BYTES + (size_t)q.T * 8);
+  MomOnly<MOM, double*> acc2;
+  if constexpr (MOM) acc2.v = acc + q.T;                  // [T] Σv² between Σv and the counts
+  uint32_t* cnt = reinterpret_cast<uint32_t*>(base + WARP_HDR_BYTES + rec_cap + STAGE_BYTES + (size_t)q.T * (MOM ? 16 : 8));
   uint8_t* scratch = base + WARP_HDR_BYTES + rec_cap + STAGE_BYTES + acc_bytes;
   if (lane == 0) { mbar_init(st.bar, 1); mbar_fence_init(); }
   __syncwarp();
@@ -347,7 +384,7 @@ scan_agg_kernel_v2(const uint8_t* __restrict__ arena, const int64_t* __restrict_
   bool have = advance_item();
   if (have) st.issue(order ? order[pos] : pos, lane);
   while (have) {
-    for (int k = lane; k < q.T; k += 32) { acc[k] = ident; cnt[k] = 0; }
+    for (int k = lane; k < q.T; k += 32) { acc[k] = ident; cnt[k] = 0; if constexpr (MOM) acc2.v[k] = 0.0; }
     __syncwarp();
     const int64_t my_item = real_item(it);
     while (true) {
@@ -366,6 +403,7 @@ scan_agg_kernel_v2(const uint8_t* __restrict__ arena, const int64_t* __restrict_
                          else if (agg_op == AGG_MAX) a = v > a ? v : a;
                          else if (agg_op != AGG_COUNT) a += v;
                          acc[k] = a; cnt[k] += 1;
+                         if constexpr (MOM) acc2.v[k] += v * v;
                        }
                      },
                      [&]() { if (inext >= 0) st.issue(inext, lane); });
@@ -381,6 +419,7 @@ scan_agg_kernel_v2(const uint8_t* __restrict__ arena, const int64_t* __restrict_
     }
     double* pv = pval + (size_t)my_item * q.T; uint32_t* pc = pcnt + (size_t)my_item * q.T;
     for (int k = lane; k < q.T; k += 32) { pv[k] = acc[k]; pc[k] = cnt[k]; }
+    if constexpr (MOM) { double* pv2 = pval2.v + (size_t)my_item * q.T; for (int k = lane; k < q.T; k += 32) pv2[k] = acc2.v[k]; }
     __syncwarp();
   }
   if (lane == 0 && (rows | bytes)) { atomicAdd(&d_counters[0], (unsigned long long)rows); atomicAdd(&d_counters[1], (unsigned long long)bytes); }
@@ -421,43 +460,49 @@ cudaError_t launch_scan_series_v2(const ScanLaunch& L, double* out, uint32_t rec
     default: return launch_series_v2_cls<CLASS_POINT>(L, out, rec_cap, smem);
   }
 }
-template <int CLS>
+template <int CLS, bool MOM>
 static cudaError_t launch_agg_v2_cls(const ScanLaunch& L, const int32_t* order, const int64_t* item_begin, int64_t n_items, int agg_op,
                                      double* pval, uint32_t* pcnt, uint32_t acc_bytes, uint32_t rec_cap, size_t smem) {
-  cudaError_t e = cudaFuncSetAttribute(scan_agg_kernel_v2<CLS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  cudaError_t e = cudaFuncSetAttribute(scan_agg_kernel_v2<CLS, MOM>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess) return e;
-  scan_agg_kernel_v2<CLS><<<L.grid, FAST_WARPS * 32, smem, L.stream>>>(L.arena, L.rec_off, order, item_begin, n_items, L.q, agg_op, pval, pcnt,
-                                                                        rec_cap, L.scratch_bytes, acc_bytes, L.d_counters, L.d_err, L.list, L.list_count);
+  scan_agg_kernel_v2<CLS, MOM><<<L.grid, FAST_WARPS * 32, smem, L.stream>>>(L.arena, L.rec_off, order, item_begin, n_items, L.q, agg_op, pval, pcnt,
+                                                                             rec_cap, L.scratch_bytes, acc_bytes, L.d_counters, L.d_err, L.list, L.list_count);
   return cudaGetLastError();
 }
-cudaError_t launch_scan_agg_v2(const ScanLaunch& L, const int32_t* order, const int64_t* item_begin, int64_t n_items, int agg_op,
-                               double* pval, uint32_t* pcnt, uint32_t acc_bytes, uint32_t rec_cap) {
-  const size_t smem = (size_t)(WARP_HDR_BYTES + rec_cap + STAGE_BYTES + acc_bytes + L.scratch_bytes) * FAST_WARPS;
+template <bool MOM>
+static cudaError_t launch_agg_v2_any(const ScanLaunch& L, const int32_t* order, const int64_t* item_begin, int64_t n_items, int agg_op,
+                                     double* pval, uint32_t* pcnt, uint32_t acc_bytes, uint32_t rec_cap, size_t smem) {
   switch (fn_class_of(L.q.fn, L.q.cumulative, L.q.long_values)) {
-    case CLASS_SUM: return launch_agg_v2_cls<CLASS_SUM>(L, order, item_begin, n_items, agg_op, pval, pcnt, acc_bytes, rec_cap, smem);
-    case CLASS_MINMAX: return launch_agg_v2_cls<CLASS_MINMAX>(L, order, item_begin, n_items, agg_op, pval, pcnt, acc_bytes, rec_cap, smem);
-    case CLASS_COUNTER: return launch_agg_v2_cls<CLASS_COUNTER>(L, order, item_begin, n_items, agg_op, pval, pcnt, acc_bytes, rec_cap, smem);
-    default: return launch_agg_v2_cls<CLASS_POINT>(L, order, item_begin, n_items, agg_op, pval, pcnt, acc_bytes, rec_cap, smem);
+    case CLASS_SUM: return launch_agg_v2_cls<CLASS_SUM, MOM>(L, order, item_begin, n_items, agg_op, pval, pcnt, acc_bytes, rec_cap, smem);
+    case CLASS_MINMAX: return launch_agg_v2_cls<CLASS_MINMAX, MOM>(L, order, item_begin, n_items, agg_op, pval, pcnt, acc_bytes, rec_cap, smem);
+    case CLASS_COUNTER: return launch_agg_v2_cls<CLASS_COUNTER, MOM>(L, order, item_begin, n_items, agg_op, pval, pcnt, acc_bytes, rec_cap, smem);
+    default: return launch_agg_v2_cls<CLASS_POINT, MOM>(L, order, item_begin, n_items, agg_op, pval, pcnt, acc_bytes, rec_cap, smem);
   }
 }
+cudaError_t launch_scan_agg_v2(const ScanLaunch& L, const int32_t* order, const int64_t* item_begin, int64_t n_items, int agg_op,
+                               double* pval, uint32_t* pcnt, uint32_t acc_bytes, uint32_t rec_cap, bool moments) {
+  const size_t smem = (size_t)(WARP_HDR_BYTES + rec_cap + STAGE_BYTES + acc_bytes + L.scratch_bytes) * FAST_WARPS;
+  return moments ? launch_agg_v2_any<true>(L, order, item_begin, n_items, agg_op, pval, pcnt, acc_bytes, rec_cap, smem)
+                 : launch_agg_v2_any<false>(L, order, item_begin, n_items, agg_op, pval, pcnt, acc_bytes, rec_cap, smem);
+}
 struct TileAggArgs { const int32_t* order; const int64_t* item_begin; int64_t n_items; int agg_op; double* pval; uint32_t* pcnt; };
-template <int FN, bool AGG>
+template <int FN, bool AGG, bool MOM>
 static cudaError_t launch_tile_fn(const ScanLaunch& L, double* out, const TileSmem& T, int64_t* fallback_list, unsigned long long* fallback_count,
                                   const TileAggArgs& A) {
-  cudaError_t e = cudaFuncSetAttribute(scan_tile_kernel<FN, AGG>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)T.total);
+  cudaError_t e = cudaFuncSetAttribute(scan_tile_kernel<FN, AGG, MOM>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)T.total);
   if (e != cudaSuccess) return e;
-  scan_tile_kernel<FN, AGG><<<L.grid, TILE_LAUNCH_THREADS, T.total, L.stream>>>(L.arena, L.rec_off, L.n_series, L.q, out, T, fallback_list, fallback_count,
+  scan_tile_kernel<FN, AGG, MOM><<<L.grid, TILE_LAUNCH_THREADS, T.total, L.stream>>>(L.arena, L.rec_off, L.n_series, L.q, out, T, fallback_list, fallback_count,
       L.d_counters, L.d_err, A.order, A.item_begin, A.n_items, A.agg_op, A.pval, A.pcnt);
   return cudaGetLastError();
 }
-template <bool AGG>
+template <bool AGG, bool MOM = false>
 static cudaError_t launch_tile_any(const ScanLaunch& L, double* out, const TileSmem& T, int64_t* fallback_list, unsigned long long* fallback_count,
                                    const TileAggArgs& A) {
   switch (L.q.fn) {
-    case FN_RATE: return launch_tile_fn<FN_RATE, AGG>(L, out, T, fallback_list, fallback_count, A);
-    case FN_AVG: return launch_tile_fn<FN_AVG, AGG>(L, out, T, fallback_list, fallback_count, A);
-    case FN_COUNT: return launch_tile_fn<FN_COUNT, AGG>(L, out, T, fallback_list, fallback_count, A);
-    default: return launch_tile_fn<FN_SUM, AGG>(L, out, T, fallback_list, fallback_count, A);      // FN_SUM, FN_INCREASE on a delta schema
+    case FN_RATE: return launch_tile_fn<FN_RATE, AGG, MOM>(L, out, T, fallback_list, fallback_count, A);
+    case FN_AVG: return launch_tile_fn<FN_AVG, AGG, MOM>(L, out, T, fallback_list, fallback_count, A);
+    case FN_COUNT: return launch_tile_fn<FN_COUNT, AGG, MOM>(L, out, T, fallback_list, fallback_count, A);
+    default: return launch_tile_fn<FN_SUM, AGG, MOM>(L, out, T, fallback_list, fallback_count, A);      // FN_SUM, FN_INCREASE on a delta schema
   }
 }
 cudaError_t launch_scan_tile(const ScanLaunch& L, double* out, const TileSmem& T, int64_t* fallback_list, unsigned long long* fallback_count) {
@@ -466,8 +511,10 @@ cudaError_t launch_scan_tile(const ScanLaunch& L, double* out, const TileSmem& T
 // fused across-series aggregate: one partial row per item (same contract as launch_scan_agg_v2); items with an irregular series
 // are appended to fallback_list
 cudaError_t launch_scan_tile_agg(const ScanLaunch& L, const TileSmem& T, const int32_t* order, const int64_t* item_begin, int64_t n_items, int agg_op,
-                                 double* pval, uint32_t* pcnt, int64_t* fallback_list, unsigned long long* fallback_count) {
-  return launch_tile_any<true>(L, nullptr, T, fallback_list, fallback_count, TileAggArgs{order, item_begin, n_items, agg_op, pval, pcnt});
+                                 double* pval, uint32_t* pcnt, int64_t* fallback_list, unsigned long long* fallback_count, bool moments) {
+  const TileAggArgs A{order, item_begin, n_items, agg_op, pval, pcnt};
+  return moments ? launch_tile_any<true, true>(L, nullptr, T, fallback_list, fallback_count, A)
+                 : launch_tile_any<true>(L, nullptr, T, fallback_list, fallback_count, A);
 }
 // v4 warp-pipeline kernel (scan_wp.cuh): one CTA of W.warps warps per SM; declined series go to fallback_list
 template <int FN, int NW>
@@ -493,36 +540,38 @@ cudaError_t launch_scan_wp(const ScanLaunch& L, double* out, const WpSmem& W, in
   }
 }
 // v4 counter-class kernel (scan_wp_ctr.cuh): per-series rows (order == nullptr, n_items == 0) or one partial row per work item
-template <int FN, bool AGG, int NW, bool IRR>
+template <int FN, bool AGG, int NW, bool IRR, bool MOM>
 static cudaError_t launch_wp_ctr_nw(const ScanLaunch& L, double* out, const WpCtrSmem& W, int64_t* fallback_list, unsigned long long* fallback_count,
                                     const TileAggArgs& A) {
   const size_t smem = (size_t)W.per_warp * W.warps + sizeof(TileCtrTab) * (TILE_CTR_TABMAX + 1);
-  cudaError_t e = cudaFuncSetAttribute(scan_wp_ctr_kernel<FN, AGG, NW, IRR>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  cudaError_t e = cudaFuncSetAttribute(scan_wp_ctr_kernel<FN, AGG, NW, IRR, MOM>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess) return e;
-  scan_wp_ctr_kernel<FN, AGG, NW, IRR><<<L.grid, W.warps * 32, smem, L.stream>>>(L.arena, L.rec_off, L.n_series, L.q, out, W, fallback_list, fallback_count,
+  scan_wp_ctr_kernel<FN, AGG, NW, IRR, MOM><<<L.grid, W.warps * 32, smem, L.stream>>>(L.arena, L.rec_off, L.n_series, L.q, out, W, fallback_list, fallback_count,
       L.d_counters, L.d_err, A.order, A.item_begin, A.n_items, A.agg_op, A.pval, A.pcnt);
   return cudaGetLastError();
 }
-template <int FN, bool AGG>
+template <int FN, bool AGG, bool MOM>
 static cudaError_t launch_wp_ctr_fn(const ScanLaunch& L, double* out, const WpCtrSmem& W, int64_t* fallback_list, unsigned long long* fallback_count, const TileAggArgs& A) {
-  if (W.tsr != 0) return launch_wp_ctr_nw<FN, AGG, 16, true>(L, out, W, fallback_list, fallback_count, A);      // irregular timestamps: the larger shared-memory footprint keeps it at <= 16 warps
-  if (W.warps <= 16) return launch_wp_ctr_nw<FN, AGG, 16, false>(L, out, W, fallback_list, fallback_count, A);
-  return launch_wp_ctr_nw<FN, AGG, WP_CTR_MAX_WARPS, false>(L, out, W, fallback_list, fallback_count, A);
+  if (W.tsr != 0) return launch_wp_ctr_nw<FN, AGG, 16, true, MOM>(L, out, W, fallback_list, fallback_count, A);      // irregular timestamps: the larger shared-memory footprint keeps it at <= 16 warps
+  if (W.warps <= 16) return launch_wp_ctr_nw<FN, AGG, 16, false, MOM>(L, out, W, fallback_list, fallback_count, A);
+  return launch_wp_ctr_nw<FN, AGG, WP_CTR_MAX_WARPS, false, MOM>(L, out, W, fallback_list, fallback_count, A);
 }
-template <bool AGG>
+template <bool AGG, bool MOM = false>
 static cudaError_t launch_wp_ctr_any(const ScanLaunch& L, double* out, const WpCtrSmem& W, int64_t* fallback_list, unsigned long long* fallback_count, const TileAggArgs& A) {
   switch (L.q.fn) {
-    case FN_RATE: return launch_wp_ctr_fn<FN_RATE, AGG>(L, out, W, fallback_list, fallback_count, A);
-    case FN_INCREASE: return launch_wp_ctr_fn<FN_INCREASE, AGG>(L, out, W, fallback_list, fallback_count, A);
-    default: return launch_wp_ctr_fn<FN_DELTA, AGG>(L, out, W, fallback_list, fallback_count, A);
+    case FN_RATE: return launch_wp_ctr_fn<FN_RATE, AGG, MOM>(L, out, W, fallback_list, fallback_count, A);
+    case FN_INCREASE: return launch_wp_ctr_fn<FN_INCREASE, AGG, MOM>(L, out, W, fallback_list, fallback_count, A);
+    default: return launch_wp_ctr_fn<FN_DELTA, AGG, MOM>(L, out, W, fallback_list, fallback_count, A);
   }
 }
 cudaError_t launch_scan_wp_ctr(const ScanLaunch& L, double* out, const WpCtrSmem& W, int64_t* fallback_list, unsigned long long* fallback_count) {
   return launch_wp_ctr_any<false>(L, out, W, fallback_list, fallback_count, TileAggArgs{nullptr, nullptr, 0, 0, nullptr, nullptr});
 }
 cudaError_t launch_scan_wp_ctr_agg(const ScanLaunch& L, const WpCtrSmem& W, const int32_t* order, const int64_t* item_begin, int64_t n_items, int agg_op,
-                                   double* pval, uint32_t* pcnt, int64_t* fallback_list, unsigned long long* fallback_count) {
-  return launch_wp_ctr_any<true>(L, nullptr, W, fallback_list, fallback_count, TileAggArgs{order, item_begin, n_items, agg_op, pval, pcnt});
+                                   double* pval, uint32_t* pcnt, int64_t* fallback_list, unsigned long long* fallback_count, bool moments) {
+  const TileAggArgs A{order, item_begin, n_items, agg_op, pval, pcnt};
+  return moments ? launch_wp_ctr_any<true, true>(L, nullptr, W, fallback_list, fallback_count, A)
+                 : launch_wp_ctr_any<true>(L, nullptr, W, fallback_list, fallback_count, A);
 }
 size_t v2_smem_per_warp(uint32_t rec_cap, uint32_t scratch_bytes, uint32_t acc_bytes) { return WARP_HDR_BYTES + (size_t)rec_cap + STAGE_BYTES + acc_bytes + scratch_bytes; }
 cudaError_t launch_scan_series(const ScanLaunch& L, double* out) {
@@ -549,7 +598,9 @@ cudaError_t launch_scan_agg(const ScanLaunch& L, const int32_t* order, const int
 cudaError_t launch_merge_partials(const double* pval, const uint32_t* pcnt, const int64_t* gis, int n_groups, int T, int agg_op,
                                   int partial_out, double* out_val, int64_t* out_cnt, cudaStream_t s) {
   const int ktiles = (T + 31) / 32;
-  merge_partials_kernel<<<n_groups * ktiles, 256, 0, s>>>(pval, pcnt, gis, n_groups, T, agg_op, partial_out, out_val, out_cnt);
+  if (agg_moments(agg_op)) merge_partials_kernel<MERGE_MOMENTS><<<n_groups * ktiles, 256, 0, s>>>(pval, pcnt, gis, n_groups, T, agg_op, partial_out, out_val, out_cnt);
+  else if (agg_op == AGG_GROUP) merge_partials_kernel<MERGE_GROUP><<<n_groups * ktiles, 256, 0, s>>>(pval, pcnt, gis, n_groups, T, agg_op, partial_out, out_val, out_cnt);
+  else merge_partials_kernel<<<n_groups * ktiles, 256, 0, s>>>(pval, pcnt, gis, n_groups, T, agg_op, partial_out, out_val, out_cnt);
   return cudaGetLastError();
 }
 cudaError_t launch_present(int agg_op, int64_t n, const double* vals, const int64_t* cnts, double* out, cudaStream_t s) {

@@ -92,8 +92,10 @@ __device__ __forceinline__ uint64_t shfl_up_u64(uint64_t v, int d) { return (uin
 
 // ---------------------------------------------------------------------------------------------------------------------
 // Tile kernel: sum/avg/count_over_time, rate/increase on delta schemas.  AGG: fused across-series aggregate (partial rows).
+// MOM (with AGG, agg_op = AGG_SUM): stddev / stdvar moments, a second register accumulator of Σv² per window, its partial rows
+// at pval + n_items * T.
 // ---------------------------------------------------------------------------------------------------------------------
-template <int FN, bool AGG>
+template <int FN, bool AGG, bool MOM = false>
 __global__ void __launch_bounds__(TILE_LAUNCH_THREADS, 2)
 scan_tile_kernel(const uint8_t* __restrict__ arena, const int64_t* __restrict__ rec_off, int64_t n_series,
                      QueryParams q, double* __restrict__ out, TileSmem L,
@@ -307,11 +309,12 @@ scan_tile_kernel(const uint8_t* __restrict__ arena, const int64_t* __restrict__ 
   const bool out_aligned = (reinterpret_cast<uintptr_t>(out) & 15) == 0;
   uint32_t parity = 0;
   int b = 0;
-  double aacc[TILE_AGG_ACC]; uint32_t acnt[TILE_AGG_ACC]; bool item_bad = false;      // AGG: this thread's windows tid + j * TILE_THREADS
+  // AGG: this thread's windows tid + j * TILE_THREADS; MOM: their Σv² at aacc[TILE_AGG_ACC + j]
+  double aacc[MOM ? 2 * TILE_AGG_ACC : TILE_AGG_ACC]; uint32_t acnt[TILE_AGG_ACC]; bool item_bad = false;
   const double agg_ident = agg_op == AGG_MIN ? __longlong_as_double(0x7ff0000000000000LL)
                          : agg_op == AGG_MAX ? __longlong_as_double(0xfff0000000000000LL) : 0.0;
 #pragma unroll
-  for (int j = 0; j < TILE_AGG_ACC; ++j) { aacc[j] = agg_ident; acnt[j] = 0; }
+  for (int j = 0; j < TILE_AGG_ACC; ++j) { aacc[j] = agg_ident; acnt[j] = 0; if constexpr (MOM) aacc[TILE_AGG_ACC + j] = 0.0; }
   int64_t rows_scanned = 0, bytes_scanned = 0, pend_rows = 0, pend_bytes = 0;
   uint32_t tj = 0;                      // tiles done by this CTA: buffer tj & 1, phase (tj >> 1) & 1 of its ready barrier
   TPROF_DECL
@@ -542,6 +545,7 @@ scan_tile_kernel(const uint8_t* __restrict__ arena, const int64_t* __restrict__ 
               const double v = otile[(size_t)s * L.out_pitch + k];
               if (v == v) {
                 if (agg_op == AGG_MIN) a = v < a ? v : a; else if (agg_op == AGG_MAX) a = v > a ? v : a; else if (agg_op != AGG_COUNT) a += v;
+                if constexpr (MOM) aacc[TILE_AGG_ACC + j] += v * v;
                 ++n;
               }
             }
@@ -554,7 +558,10 @@ scan_tile_kernel(const uint8_t* __restrict__ arena, const int64_t* __restrict__ 
 #pragma unroll
           for (int j = 0; j < TILE_AGG_ACC; ++j) {
             const int k = tid + j * TILE_THREADS;
-            if (k < q.T) { pval[(size_t)w.it * q.T + k] = aacc[j]; pcnt[(size_t)w.it * q.T + k] = acnt[j]; }
+            if (k < q.T) {
+              pval[(size_t)w.it * q.T + k] = aacc[j]; pcnt[(size_t)w.it * q.T + k] = acnt[j];
+              if constexpr (MOM) pval[(size_t)(n_items + w.it) * q.T + k] = aacc[TILE_AGG_ACC + j];
+            }
           }
           rows_scanned += pend_rows; bytes_scanned += pend_bytes;
         } else if (tid == 0) {
@@ -563,7 +570,7 @@ scan_tile_kernel(const uint8_t* __restrict__ arena, const int64_t* __restrict__ 
         }
         pend_rows = 0; pend_bytes = 0;
 #pragma unroll
-        for (int j = 0; j < TILE_AGG_ACC; ++j) { aacc[j] = agg_ident; acnt[j] = 0; }
+        for (int j = 0; j < TILE_AGG_ACC; ++j) { aacc[j] = agg_ident; acnt[j] = 0; if constexpr (MOM) aacc[TILE_AGG_ACC + j] = 0.0; }
         item_bad = false;
       }
     } else {

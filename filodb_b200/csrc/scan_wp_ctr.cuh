@@ -189,7 +189,9 @@ __device__ __forceinline__ double wp_clamped_window(const double* V, const WpCtr
 }
 
 // IRR: the table has timestamp vectors off the step grid (its own instantiation: the regular kernel keeps its code and register budget)
-template <int FN, bool AGG, int NW, bool IRR = false>
+// MOM (with AGG, agg_op = AGG_SUM): stddev / stdvar moments, a second [T] row of Σv² in the warp's region behind the NaN counts
+// (wp_ctr_layout sizes it only for this mode), its partial rows at pval + n_items * T
+template <int FN, bool AGG, int NW, bool IRR = false, bool MOM = false>
 __global__ void __launch_bounds__(NW * 32, 1)
 scan_wp_ctr_kernel(const uint8_t* __restrict__ arena, const int64_t* __restrict__ rec_off, int64_t n_series, QueryParams q,
                    double* __restrict__ out, WpCtrSmem L, int64_t* __restrict__ fallback_list, unsigned long long* __restrict__ fallback_count,
@@ -208,6 +210,8 @@ scan_wp_ctr_kernel(const uint8_t* __restrict__ arena, const int64_t* __restrict_
   double* V = reinterpret_cast<double*>(wb + L.vals);
   WpCtrChunk* KC = reinterpret_cast<WpCtrChunk*>(wb + L.kc);
   double* ACC = reinterpret_cast<double*>(wb + L.acc);
+  MomOnly<MOM, double*> ACC2;
+  if constexpr (MOM) ACC2.v = reinterpret_cast<double*>(wb + L.nbad + align_up((uint32_t)q.T * 2u, 16));
   uint16_t* NBAD = reinterpret_cast<uint16_t*>(wb + L.nbad);
   int32_t* TSR = reinterpret_cast<int32_t*>(wb + L.tsr);                 // (L.tsr == 0: tables with const-DDV timestamps only; never read then)
   constexpr bool allow_irr = IRR;
@@ -258,7 +262,7 @@ scan_wp_ctr_kernel(const uint8_t* __restrict__ arena, const int64_t* __restrict_
   if (more) { cur_sid = sid_at(c_p); cur_off = rec_off[cur_sid]; cur_sz = (uint32_t)(rec_off[cur_sid + 1] - cur_off); }
   if (more && cur_sz <= L.rec_cap && lane == 0) issue(cur_off, cur_sz);
   bool item_bad = false; int item_nser = 0;
-  if (AGG) { for (int k = lane; k < q.T; k += 32) { ACC[k] = agg_ident; NBAD[k] = 0; } __syncwarp(); }
+  if (AGG) { for (int k = lane; k < q.T; k += 32) { ACC[k] = agg_ident; NBAD[k] = 0; if constexpr (MOM) ACC2.v[k] = 0.0; } __syncwarp(); }
 
   while (more) {
     // successor in walk order (its record is fetched as soon as R is dead)
@@ -421,6 +425,7 @@ scan_wp_ctr_kernel(const uint8_t* __restrict__ arena, const int64_t* __restrict_
         if (v == v) {                                        // RowAggregators skip NaN (SumRowAggregator.scala:22-29 ...)
           if (agg_add) ACC[k] += v;
           else if (agg_op != AGG_COUNT) { const double a = ACC[k]; if (agg_op == AGG_MIN ? v < a : v > a) ACC[k] = v; }
+          if constexpr (MOM) ACC2.v[k] += v * v;
         } else wp_bump_u16(NBAD + k);
       };
       for (int ci = 0; ci < n; ++ci) {
@@ -504,11 +509,12 @@ scan_wp_ctr_kernel(const uint8_t* __restrict__ arena, const int64_t* __restrict_
         if (!item_bad) {
           double* pv = pval + (size_t)c_it * q.T; uint32_t* pc = pcnt + (size_t)c_it * q.T;
           for (int k = lane; k < q.T; k += 32) { pv[k] = ACC[k]; pc[k] = (uint32_t)(item_nser - (int)NBAD[k]); }
+          if constexpr (MOM) { double* pv2 = pval + (size_t)(n_items + c_it) * q.T; for (int k = lane; k < q.T; k += 32) pv2[k] = ACC2.v[k]; }
           if (lane == 0) { rows_scanned += pend_rows; bytes_scanned += pend_bytes; }
         } else if (lane == 0) {
           const unsigned long long slot = atomicAdd(fallback_count, 1ull); fallback_list[slot] = c_it;
         }
-        for (int k = lane; k < q.T; k += 32) { ACC[k] = agg_ident; NBAD[k] = 0; }
+        for (int k = lane; k < q.T; k += 32) { ACC[k] = agg_ident; NBAD[k] = 0; if constexpr (MOM) ACC2.v[k] = 0.0; }
         pend_rows = 0; pend_bytes = 0; item_bad = false; item_nser = 0;
       }
     }

@@ -98,7 +98,8 @@ struct WpCtrSmem {                     // byte offsets inside a warp's region (m
 };
 constexpr uint32_t WP_OFF_DROPS = WP_OFF_J + 64 * 8;          // TileDrops[WP_MAXC] behind the 64-word XOR prefix table
 static_assert(WP_OFF_DROPS + WP_MAXC * sizeof(TileDrops) <= WP_OFF_REC, "drops fit in front of the record");
-FILO_HD inline WpCtrSmem wp_ctr_layout(uint32_t max_rec_bytes, uint32_t max_rows, uint32_t max_chunks, uint32_t T, bool agg, bool irr = false) {
+FILO_HD inline WpCtrSmem wp_ctr_layout(uint32_t max_rec_bytes, uint32_t max_rows, uint32_t max_chunks, uint32_t T, bool agg, bool irr = false,
+                                       bool moments = false) {
   WpCtrSmem L;
   if (max_chunks > (uint32_t)WP_MAXC) max_chunks = WP_MAXC;
   L.rec_cap = align_up(max_rec_bytes + 16, 16);
@@ -111,6 +112,7 @@ FILO_HD inline WpCtrSmem wp_ctr_layout(uint32_t max_rec_bytes, uint32_t max_rows
   if (irr) { L.tsr = o; o += align_up(P * 4, 16); }
   L.acc = o; L.nbad = o;
   if (agg) { o += T * 8; L.nbad = o; o += align_up(T * 2, 16); }
+  if (agg && moments) o += T * 8;      // stddev / stdvar: the [T] Σv² row at nbad + align_up(T * 2, 16)
   L.per_warp = align_up(o, 16);
   L.tab = 0; L.warps = 0; L.agg = agg ? 1u : 0u;
   return L;

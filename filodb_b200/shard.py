@@ -9,7 +9,7 @@ Works on CUDA tensors over NCCL (product) and on CPU tensors over gloo (tests/te
 """
 from __future__ import annotations
 
-AGG_NONE, AGG_SUM, AGG_AVG, AGG_MIN, AGG_MAX, AGG_COUNT, AGG_TOPK, AGG_BOTTOMK = range(8)
+AGG_NONE, AGG_SUM, AGG_AVG, AGG_MIN, AGG_MAX, AGG_COUNT, AGG_TOPK, AGG_BOTTOMK, AGG_STDDEV, AGG_STDVAR, AGG_GROUP = range(11)
 
 
 def shards_of_rank(num_shards: int, rank: int, world: int) -> list[int]:
@@ -30,9 +30,10 @@ def series_range_of_rank(n_series_total: int, rank: int, world: int) -> tuple[in
 
 
 def merge_partials(values, counts, aggr_op: int, dist) -> None:
-    """In-place cross-rank merge of FILO_Q_PARTIAL results: values [G*T] f64, counts [G*T] i64.
-    sum/avg/count: Σ values, Σ counts; min/max: min/max of values (identity ±Inf), Σ counts."""
-    if aggr_op in (AGG_SUM, AGG_AVG, AGG_COUNT):
+    """In-place cross-rank merge of FILO_Q_PARTIAL results: values [G*T] f64 ([2*G*T] for stddev / stdvar: the Σv and Σv² blocks),
+    counts [G*T] i64.  sum/avg/count/group: Σ values, Σ counts; stddev/stdvar: Σ of both value blocks, Σ counts (the moments add up);
+    min/max: min/max of values (identity ±Inf), Σ counts."""
+    if aggr_op in (AGG_SUM, AGG_AVG, AGG_COUNT, AGG_GROUP, AGG_STDDEV, AGG_STDVAR):
         dist.all_reduce(values, op=dist.ReduceOp.SUM)
     elif aggr_op == AGG_MIN:
         dist.all_reduce(values, op=dist.ReduceOp.MIN)

@@ -82,7 +82,11 @@ enum {
 /* AggregationOperator subset (query/src/main/scala/filodb/query/PlanEnums.scala:99-114) */
 enum {
   FILO_AGG_NONE = 0, FILO_AGG_SUM = 1, FILO_AGG_AVG = 2, FILO_AGG_MIN = 3, FILO_AGG_MAX = 4,
-  FILO_AGG_COUNT = 5, FILO_AGG_TOPK = 6, FILO_AGG_BOTTOMK = 7
+  FILO_AGG_COUNT = 5, FILO_AGG_TOPK = 6, FILO_AGG_BOTTOMK = 7,
+  /* RowAggregator.apply (aggregator/RowAggregator.scala:133,138-139): StddevRowAggregator.scala:39-58,
+   * StdvarRowAggregator.scala:52-72 (sumSquare/count - mean^2, sqrt of it for stddev), GroupRowAggregator.scala:23-29
+   * (1.0 where any input is non-NaN).  Scalar tables only: histogram tables answer FILO_ERR_UNSUPPORTED. */
+  FILO_AGG_STDDEV = 8, FILO_AGG_STDVAR = 9, FILO_AGG_GROUP = 10
 };
 
 /* schema_flags of filo_load_series */
@@ -217,8 +221,11 @@ void    filo_table_free(filo_ctx* ctx, filo_table* t);
 int32_t filo_num_windows(int64_t start_ms, int64_t step_ms, int64_t end_ms);
 
 /* PeriodicSamplesMapper (+ AggregateMapReduce when aggr_op != NONE) over a loaded table; results to HOST buffers.
- *  out_values: aggr NONE -> [n_series * T]; SUM/AVG/MIN/MAX/COUNT -> [n_groups * T]; TOPK/BOTTOMK -> [n_groups * T * k]
- *  out_aux:    AVG -> counts [n_groups*T]; TOPK/BOTTOMK -> series ordinals [n_groups*T*k] (-1 = empty); else may be NULL */
+ *  out_values: aggr NONE -> [n_series * T]; SUM/AVG/MIN/MAX/COUNT/STDDEV/STDVAR/GROUP -> [n_groups * T]; TOPK/BOTTOMK -> [n_groups * T * k];
+ *              STDDEV/STDVAR with FILO_Q_PARTIAL -> [2 * n_groups * T] (see filo_query_device)
+ *  out_aux:    AVG -> counts [n_groups*T]; TOPK/BOTTOMK -> series ordinals [n_groups*T*k] (-1 = empty); else may be NULL
+ *  STDVAR presents NaN where no input is non-NaN, else Σv²/n - m*m with m = Σv/n; STDDEV presents sqrt of that, NaN when the
+ *  variance rounds below zero (Math.pow(negative, 0.5)); GROUP presents 1.0 or NaN.  Their counts go to out_aux when it is not NULL. */
 int32_t filo_query(filo_ctx* ctx, const filo_table* t, int32_t range_fn,
                    int64_t start_ms, int64_t step_ms, int64_t end_ms, int64_t window_ms,
                    int32_t aggr_op, int32_t k, int32_t flags,
@@ -227,7 +234,12 @@ int32_t filo_query(filo_ctx* ctx, const filo_table* t, int32_t range_fn,
  * (a cudaStream_t, may be NULL = ctx stream); does not synchronize unless stats != NULL.
  * With FILO_Q_PARTIAL: SUM/AVG/COUNT -> values = Σ of non-NaN inputs (0 when none), aux = contributing count;
  * MIN/MAX -> values = min/max with +Inf/-Inf identity, aux = count.  Merge across GPUs with ncclSum / ncclMin /
- * ncclMax on values and ncclSum on aux, then call filo_present_partials. */
+ * ncclMax on values and ncclSum on aux, then call filo_present_partials.
+ * STDDEV/STDVAR with FILO_Q_PARTIAL -> values = [2 * n_groups * T]: the Σv block, then the Σv² block (0 when no input), aux = count
+ * (required); both blocks merge with ncclSum.  GROUP with FILO_Q_PARTIAL is exactly the COUNT partial.  For a cross-node
+ * ReduceAggregateExec the adapter turns a (Σv, Σv², n) cell into the reference's reduction schema (stdvar|stddev, mean, count)
+ * (StdvarRowAggregator.scala:76-79): mean = Σv/n, stdvar = Σv²/n - mean*mean (stddev = sqrt of it), count = n; a cell with n = 0
+ * becomes (NaN, NaN, 0). */
 int32_t filo_query_device(filo_ctx* ctx, const filo_table* t, int32_t range_fn,
                           int64_t start_ms, int64_t step_ms, int64_t end_ms, int64_t window_ms,
                           int32_t aggr_op, int32_t k, int32_t flags,
@@ -275,7 +287,8 @@ int32_t filo_scan_series(filo_ctx* ctx, int64_t n_series, const int32_t* n_chunk
                          int32_t ts_col, int32_t val_col, int32_t schema_flags,
                          int32_t range_fn, int64_t start_ms, int64_t step_ms, int64_t end_ms, int64_t window_ms,
                          double* out_values, filo_stats* stats);
-/* RowAggregator "present" after a cross-GPU merge: n = n_groups*T cells; writes NaN where count == 0, Σ/n for AVG. */
+/* RowAggregator "present" after a cross-GPU merge: n = n_groups*T cells; writes NaN where count == 0, Σ/n for AVG.
+ * STDDEV/STDVAR read the Σv² block at d_values + n (the FILO_Q_PARTIAL layout); GROUP writes 1.0 where count > 0. */
 int32_t filo_present_partials(filo_ctx* ctx, int32_t aggr_op, int64_t n, void* d_values, void* d_counts,
                               void* d_out_values, void* cuda_stream);
 

@@ -42,7 +42,7 @@ enum class InternalRangeFunction : int32_t {
 // AggregationOperator (query/src/main/scala/filodb/query/PlanEnums.scala) subset
 enum class AggregationOperator : int32_t {
   Sum = FILO_AGG_SUM, Avg = FILO_AGG_AVG, Min = FILO_AGG_MIN, Max = FILO_AGG_MAX, Count = FILO_AGG_COUNT,
-  TopK = FILO_AGG_TOPK, BottomK = FILO_AGG_BOTTOMK
+  TopK = FILO_AGG_TOPK, BottomK = FILO_AGG_BOTTOMK, Stddev = FILO_AGG_STDDEV, Stdvar = FILO_AGG_STDVAR, Group = FILO_AGG_GROUP
 };
 
 // RawDataRangeVector: one partition's chunks for the query range (ChunkSetInfo native addresses in chunkID order) + the group
