@@ -126,8 +126,9 @@ scan_agg_kernel(const uint8_t* __restrict__ arena, const int64_t* __restrict__ r
         const double v = eval_window(D, 0, n, q, k);
         if (v == v) {                                       // RowAggregators skip NaN (SumRowAggregator.scala:22-29 ...)
           double a = acc[k];
-          if (agg_op == AGG_MIN) a = v < a ? v : a;
-          else if (agg_op == AGG_MAX) a = v > a ? v : a;
+          // min/maxIgnoreNaN(acc, v) (QueryUtils.scala:111-123): of two equal values (+0.0 / -0.0) the later one is kept
+          if (agg_op == AGG_MIN) a = a < v ? a : v;
+          else if (agg_op == AGG_MAX) a = a > v ? a : v;
           else if (agg_op == AGG_COUNT) a = a;             // count only
           else a += v;
           acc[k] = a; cnt[k] += 1;
@@ -146,6 +147,9 @@ scan_agg_kernel(const uint8_t* __restrict__ arena, const int64_t* __restrict__ r
 
 // Fold the partial rows of each group (items [gis[g], gis[g+1])) in item order.  Block = (32 windows) x (8 item lanes);
 // thread (kk, j) folds items j, j+8, ... sequentially, then the 8 lanes are folded in fixed order -> deterministic.
+// MIN / MAX fold as min/maxIgnoreNaN(acc, v) (QueryUtils.scala:111-123): of equal values (+0.0 / -0.0) the later one is kept.  That
+// rule is associative, so the tree equals one sequential fold over the items in the order 0, 8, 16, ..., 1, 9, 17, ..., 7, 15, ...,
+// with each item's series folded in group order by the scan kernel.
 // partial_out: values/counts in mergeable form; otherwise presented (NaN when count == 0; Σ/n for AVG; n for COUNT).
 // EXT = MERGE_MOMENTS (STDDEV/STDVAR): the Σv² rows follow the Σv rows (pval + n_items * T, n_items = gis[n_groups]) and are folded
 // by the same tree; their mergeable form is [2][n_groups][T].  EXT = MERGE_GROUP: the count partial, presented as 1.0 / NaN.
@@ -188,7 +192,7 @@ merge_partials_kernel(const double* __restrict__ pval, const uint32_t* __restric
     for (int64_t it = gis[g] + j; it < gis[g + 1]; it += 8) {
       const double v = pval[(size_t)it * T + k]; const uint32_t n = pcnt[(size_t)it * T + k];
       if (n) {
-        if (agg_op == AGG_MIN) a = v < a ? v : a; else if (agg_op == AGG_MAX) a = v > a ? v : a; else a += v;
+        if (agg_op == AGG_MIN) a = a < v ? a : v; else if (agg_op == AGG_MAX) a = a > v ? a : v; else a += v;
         if constexpr (MOM) a2.v += pval[(size_t)(gis[n_groups] + it) * T + k];
         c += n;
       }
@@ -200,7 +204,7 @@ merge_partials_kernel(const double* __restrict__ pval, const uint32_t* __restric
   if (j == 0 && k < T) {
     for (int jj = 1; jj < 8; ++jj) {
       const double v = sv[jj][kk]; const unsigned long long n = sc[jj][kk];
-      if (n) { if (agg_op == AGG_MIN) a = v < a ? v : a; else if (agg_op == AGG_MAX) a = v > a ? v : a; else a += v; c += n; }
+      if (n) { if (agg_op == AGG_MIN) a = a < v ? a : v; else if (agg_op == AGG_MAX) a = a > v ? a : v; else a += v; c += n; }
     }
     const size_t o = (size_t)g * T + k;
     if constexpr (EXT != MERGE_PLAIN) {
@@ -399,8 +403,9 @@ scan_agg_kernel_v2(const uint8_t* __restrict__ arena, const int64_t* __restrict_
                      [&](int k, double v, bool valid) {
                        if (valid && v == v) {              // RowAggregators skip NaN (SumRowAggregator.scala:22-29 ...)
                          double a = acc[k];
-                         if (agg_op == AGG_MIN) a = v < a ? v : a;
-                         else if (agg_op == AGG_MAX) a = v > a ? v : a;
+                         // min/maxIgnoreNaN(acc, v) (QueryUtils.scala:111-123): of two equal values the later one is kept
+                         if (agg_op == AGG_MIN) a = a < v ? a : v;
+                         else if (agg_op == AGG_MAX) a = a > v ? a : v;
                          else if (agg_op != AGG_COUNT) a += v;
                          acc[k] = a; cnt[k] += 1;
                          if constexpr (MOM) acc2.v[k] += v * v;

@@ -544,7 +544,8 @@ scan_tile_kernel(const uint8_t* __restrict__ arena, const int64_t* __restrict__ 
             for (int s = 0; s < ns; ++s) {
               const double v = otile[(size_t)s * L.out_pitch + k];
               if (v == v) {
-                if (agg_op == AGG_MIN) a = v < a ? v : a; else if (agg_op == AGG_MAX) a = v > a ? v : a; else if (agg_op != AGG_COUNT) a += v;
+                // min/maxIgnoreNaN(acc, v) (QueryUtils.scala:111-123): of two equal values the later one is kept
+                if (agg_op == AGG_MIN) a = a < v ? a : v; else if (agg_op == AGG_MAX) a = a > v ? a : v; else if (agg_op != AGG_COUNT) a += v;
                 if constexpr (MOM) aacc[TILE_AGG_ACC + j] += v * v;
                 ++n;
               }

@@ -424,7 +424,9 @@ scan_wp_ctr_kernel(const uint8_t* __restrict__ arena, const int64_t* __restrict_
         if (!AGG) { wp_store_result(gout + k, v); return; }
         if (v == v) {                                        // RowAggregators skip NaN (SumRowAggregator.scala:22-29 ...)
           if (agg_add) ACC[k] += v;
-          else if (agg_op != AGG_COUNT) { const double a = ACC[k]; if (agg_op == AGG_MIN ? v < a : v > a) ACC[k] = v; }
+          // acc = min/maxIgnoreNaN(acc, v) (QueryUtils.scala:111-123): v replaces acc unless acc is strictly better, so of two equal
+          // values (+0.0 / -0.0) the later one is kept
+          else if (agg_op != AGG_COUNT) { const double a = ACC[k]; if (agg_op == AGG_MIN ? !(a < v) : !(a > v)) ACC[k] = v; }
           if constexpr (MOM) ACC2.v[k] += v * v;
         } else wp_bump_u16(NBAD + k);
       };

@@ -22,18 +22,10 @@ struct SeriesData { std::vector<std::unique_ptr<Chunk>> chunks; std::vector<uint
 static long g_wp_declined = 0, g_wp_series = 0;
 static int g_long_col = 0;          // 1: Long value column through LongBinaryVector.optimize (DDV / const DDV), 2: raw 64-bit longs
 static int g_jitter_ms = 0; static bool g_integral = false;      // irregular scrapes (DDV timestamps) / integral values (DoubleVector.optimize -> DDV longs)
-static void build_series(SeriesData& S, std::mt19937_64& rng, int rows, const std::vector<int>& chunk_rows, int64_t t0, int step_ms, int kind /*0 gauge 1 counter*/,
-                         bool xor_enc, int nan_ppm, int reset_every) {
-  std::vector<int64_t> ts((size_t)rows); std::vector<double> v((size_t)rows);
-  std::normal_distribution<double> N(0.0, 1.0);
-  double acc = 0.0;
-  for (int r = 0; r < rows; ++r) {
-    ts[(size_t)r] = t0 + (int64_t)r * step_ms + (g_jitter_ms ? (int64_t)(rng() % (uint64_t)(2 * g_jitter_ms + 1)) - g_jitter_ms : 0);
-    double g = 15.0 + std::sin((double)(r + 1)) + N(rng);
-    if (g_integral) g = std::floor(g);
-    if (kind == 0) v[(size_t)r] = g;
-    else { if (reset_every && r > 0 && rng() % (uint64_t)reset_every == 0) acc = 0.0; acc += g > 0 ? g : 0.0; v[(size_t)r] = acc; }
-  }
+static bool g_signed_zero = false;  // gauge values +0.0 / -0.0 in runs of 12 rows: min / max meet equal zeros of both signs
+// chunks of the given rows (nan_ppm: a stale marker at a chunk end) and the arena record, from timestamps and values
+static void build_series_from(SeriesData& S, std::mt19937_64& rng, const std::vector<int64_t>& ts, const std::vector<double>& v, const std::vector<int>& chunk_rows,
+                              int kind /*0 gauge 1 counter*/, bool xor_enc, int nan_ppm) {
   int r0 = 0;
   for (int n : chunk_rows) {
     auto c = std::make_unique<Chunk>();
@@ -78,6 +70,21 @@ static void build_series(SeriesData& S, std::mt19937_64& rng, int rows, const st
   std::memcpy(S.record.data(), &h, sizeof h);
   std::memcpy(S.record.data() + sizeof h, E.data(), nch * sizeof(filo::ChunkEntry));
   std::memcpy(S.record.data() + off, body.data(), body.size());
+}
+static void build_series(SeriesData& S, std::mt19937_64& rng, int rows, const std::vector<int>& chunk_rows, int64_t t0, int step_ms, int kind /*0 gauge 1 counter*/,
+                         bool xor_enc, int nan_ppm, int reset_every) {
+  std::vector<int64_t> ts((size_t)rows); std::vector<double> v((size_t)rows);
+  std::normal_distribution<double> N(0.0, 1.0);
+  double acc = 0.0, zrun = 0.0;
+  for (int r = 0; r < rows; ++r) {
+    ts[(size_t)r] = t0 + (int64_t)r * step_ms + (g_jitter_ms ? (int64_t)(rng() % (uint64_t)(2 * g_jitter_ms + 1)) - g_jitter_ms : 0);
+    double g = 15.0 + std::sin((double)(r + 1)) + N(rng);
+    if (g_integral) g = std::floor(g);
+    if (g_signed_zero) { if (r % 12 == 0) zrun = rng() & 1 ? -0.0 : 0.0; g = zrun; }
+    if (kind == 0) v[(size_t)r] = g;
+    else { if (reset_every && r > 0 && rng() % (uint64_t)reset_every == 0) acc = 0.0; acc += g > 0 ? g : 0.0; v[(size_t)r] = acc; }
+  }
+  build_series_from(S, rng, ts, v, chunk_rows, kind, xor_enc, nan_ppm);
 }
 
 static bool same_bits(double a, double b) { uint64_t x, y; std::memcpy(&x, &a, 8); std::memcpy(&y, &b, 8); return x == y || (a != a && b != b); }
@@ -154,7 +161,7 @@ int main(int argc, char** argv) {
   std::mt19937_64 rng(4242);
   long checked = 0; int cases = 0;
   struct Cfg { int kind = 0; bool xor_enc = true; int fn = 0; std::vector<int> chunks; int nan_ppm = 0, reset_every = 0; int64_t window = 300000; int nser = 1; int inclusive = 1;
-               int64_t start_off = 0, end_off = 0; int agg_op = 0; int grid = 1; int jitter = 0; bool integral = false; bool v2_only = false; bool wp = false; bool hetero = false; int long_col = 0; double p0 = 0, p1 = 0; };
+               int64_t start_off = 0, end_off = 0; int agg_op = 0; int grid = 1; int jitter = 0; bool integral = false; bool v2_only = false; bool wp = false; bool hetero = false; int long_col = 0; double p0 = 0, p1 = 0; bool szero = false; };
   std::vector<Cfg> all_ext;
   const std::vector<Cfg> cfgs = {
     {0, true, filo::FN_RATE, {400, 80}, 200000, 0, 300000, 11, 1, 0, 0, 0, 2},           // C2: gauge, delta-temporality rate (CLASS_SUM), NaN stale markers
@@ -209,6 +216,9 @@ int main(int argc, char** argv) {
     // tile kernel + fallback pass: irregular scrapes make the tile kernel decline every series
     {0, true, filo::FN_RATE, {200, 100}, 0, 0, 300000, 10, 1, 0, 0, 0, 2, 4000, false, false},
     {0, true, filo::FN_RATE, {400, 80}, 100000, 0, 300000, 26, 1, 0, 0, filo::AGG_SUM, 2},   // fused sum: items of 5 series in shuffled order
+    // fused min / max over +0.0 / -0.0 gauges (delta: the v4 counter kernel): of equal values the later one is kept (QueryUtils.scala:111-123)
+    {0, true, filo::FN_DELTA, {400, 80}, 0, 0, 300000, 26, 1, 0, 0, filo::AGG_MIN, 2, 0, false, false, false, false, 0, 0, 0, true},
+    {0, false, filo::FN_DELTA, {400, 80}, 0, 0, 300000, 26, 1, 0, 0, filo::AGG_MAX, 2, 0, false, false, false, false, 0, 0, 0, true},
   };
   // the remaining chunked range functions and the Long-column variants: window by window on the v2 kernel (eval_window_ext)
   {
@@ -275,7 +285,7 @@ int main(int argc, char** argv) {
     const int64_t t0 = 1700000000000LL; const int step_ms = 15000;
     std::vector<SeriesData> SS((size_t)c.nser);
     std::vector<int64_t> rec_off((size_t)c.nser + 1, 0);
-    g_jitter_ms = c.jitter; g_integral = c.integral; g_long_col = c.long_col;
+    g_jitter_ms = c.jitter; g_integral = c.integral; g_long_col = c.long_col; g_signed_zero = c.szero;
     for (int s = 0; s < c.nser; ++s) {
       std::vector<int> cr = c.chunks; int64_t ts0 = t0; bool xe = c.xor_enc;
       if (c.hetero) {      // series-dependent chunk split, start time and encoding (runs of equal shapes in between)
@@ -400,7 +410,7 @@ int main(int argc, char** argv) {
           double a = c.agg_op == filo::AGG_MIN ? INFINITY : c.agg_op == filo::AGG_MAX ? -INFINITY : 0.0; uint32_t n = 0;
           for (int64_t p = item_begin[(size_t)it]; p < item_begin[(size_t)it + 1]; ++p) {
             const double v = ref[(size_t)order[(size_t)p] * q.T + k];
-            if (v == v) { if (c.agg_op == filo::AGG_MIN) a = v < a ? v : a; else if (c.agg_op == filo::AGG_MAX) a = v > a ? v : a; else if (c.agg_op != filo::AGG_COUNT) a += v; ++n; }
+            if (v == v) { if (c.agg_op == filo::AGG_MIN) a = fo::minIgnoreNaN(a, v); else if (c.agg_op == filo::AGG_MAX) a = fo::maxIgnoreNaN(a, v); else if (c.agg_op != filo::AGG_COUNT) a += v; ++n; }
           }
           if (!same_bits(pval[(size_t)it * q.T + k], a) || pcnt[(size_t)it * q.T + k] != n) { std::printf("FAIL cfg %zu item %lld window %d: %.17g (%u) vs %.17g (%u)\n", ci, (long long)it, k, pval[(size_t)it * q.T + k], pcnt[(size_t)it * q.T + k], a, n); return 1; }
           ++checked;
@@ -418,11 +428,11 @@ int main(int argc, char** argv) {
           for (int j = 0; j < 8; ++j) {
             double a = ident; unsigned long long n = 0;
             for (int64_t it = j; it < n_items; it += 8) { const double v = pval[(size_t)it * q.T + k]; const uint32_t m = pcnt[(size_t)it * q.T + k];
-              if (m) { if (c.agg_op == filo::AGG_MIN) a = v < a ? v : a; else if (c.agg_op == filo::AGG_MAX) a = v > a ? v : a; else a += v; n += m; } }
+              if (m) { if (c.agg_op == filo::AGG_MIN) a = fo::minIgnoreNaN(a, v); else if (c.agg_op == filo::AGG_MAX) a = fo::maxIgnoreNaN(a, v); else a += v; n += m; } }
             lane_a[j] = a; lane_c[j] = n;
           }
           double a = lane_a[0]; unsigned long long n = lane_c[0];
-          for (int j = 1; j < 8; ++j) if (lane_c[j]) { const double v = lane_a[j]; if (c.agg_op == filo::AGG_MIN) a = v < a ? v : a; else if (c.agg_op == filo::AGG_MAX) a = v > a ? v : a; else a += v; n += lane_c[j]; }
+          for (int j = 1; j < 8; ++j) if (lane_c[j]) { const double v = lane_a[j]; if (c.agg_op == filo::AGG_MIN) a = fo::minIgnoreNaN(a, v); else if (c.agg_op == filo::AGG_MAX) a = fo::maxIgnoreNaN(a, v); else a += v; n += lane_c[j]; }
           const double e = n == 0 ? std::nan("") : c.agg_op == filo::AGG_AVG ? a / (double)n : c.agg_op == filo::AGG_COUNT ? (double)n : a;
           if (!same_bits(mv[(size_t)k], e) || mc[(size_t)k] != (int64_t)n) { std::printf("FAIL cfg %zu merged window %d: %.17g (%lld) vs %.17g (%llu)\n", ci, k, mv[(size_t)k], (long long)mc[(size_t)k], e, n); return 1; }
           ++checked;

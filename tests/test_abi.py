@@ -120,10 +120,10 @@ def test_scan_kernels_run_on_the_simt_emulator(tmp_path):
                     os.path.join(ROOT, "tests", "cpp", "tile_emul.cpp"), "-o", exe], check=True)
     for seed in ("0", "20260922"):
         out = subprocess.run([exe, seed], check=True, capture_output=True, text=True).stdout
-        assert "OK 102 cases" in out and "bit-exact" in out, out
+        assert "OK 104 cases" in out and "bit-exact" in out, out
     # random shapes: chunk counts and sizes, windows, offsets, functions, NaN / reset rates, per-series and fused modes
     out = subprocess.run([exe, "7", "fuzz", "60"], check=True, capture_output=True, text=True).stdout
-    assert "OK 162 cases" in out and "bit-exact" in out, out
+    assert "OK 164 cases" in out and "bit-exact" in out, out
 
 
 def test_histogram_kernels_run_on_the_simt_emulator(tmp_path):

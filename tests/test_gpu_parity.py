@@ -34,8 +34,10 @@ def same_bits(a, b):
 
 def assert_same(a, b, what=""):
     if not same_bits(a, b):
-        a = np.asarray(a); b = np.asarray(b)
-        bad = np.argwhere(~((a == b) | (np.isnan(a) & np.isnan(b))))
+        a = np.ascontiguousarray(a, np.float64); b = np.ascontiguousarray(b, np.float64)
+        if a.shape != b.shape:
+            raise AssertionError("%s: shapes %s vs %s" % (what, a.shape, b.shape))
+        bad = np.argwhere(~((a.view(np.uint64) == b.view(np.uint64)) | (np.isnan(a) & np.isnan(b))))      # bits: +0.0 != -0.0
         i = tuple(bad[0])
         raise AssertionError("%s: %d mismatches, first at %s: gpu=%r oracle=%r" % (what, len(bad), i, a[i], b[i]))
 
