@@ -8,16 +8,19 @@
 //      (x + 0.0 == x for every sum of non-zero values and +0.0 rows), skewed by one pad slot per 8 rows: both the 8-byte row stores of the
 //      group decode (lane stride 8 rows) and the 8-byte row loads of the window blocks (lane stride 8 windows) then walk the banks with
 //      an odd stride of 9 words -- conflict-free;
-//   O  the series' T results, in V's place when the plan allows it; they leave as lane-consecutive streaming stores (256 contiguous
-//      bytes per store instruction) once every window is finished.
+//   O  the series' window sums, in V's place when the plan allows it: finished values, or raw sums still to be finished.
 // Phases of a series (all 32 lanes, only __syncwarp between them):
-//   setup    lane c = chunk c: header parse, regularity checks, window plan (touch interval, block list, row positions).  The plan
-//            depends on (init, nrows, endTime) of the chunks only, so it is reused while consecutive series share those (memo);
+//   setup    lane c = chunk c: header parse, regularity checks, window plan (touch interval, block list, row positions, and the class
+//            of every window a lane stores, see wp_class).  The plan depends on (init, nrows, endTime) of the chunks only, so it is
+//            reused while consecutive series share those (memo);
 //   decode   lane = NibblePack group (two groups per lane): branch-free field extraction, XOR prefix inside the group, warp-wide
 //            XOR scan over the group totals, rows stored once;
 //   windows  item = (chunk, block of 8 windows), two items per lane: register-blocked sequential sums in the reference's row order
 //            (DoubleVector.scala:243-253, AggrOverTimeFunctions.scala:560-571).  A window that takes rows from two chunks gets one
-//            partial sum from each chunk's block list; a short fix-up pass adds them in chunk order.
+//            partial sum from each chunk's block list (the earlier chunk's in O, the later one's in J);
+//   finish   lane l = windows l + 32 m: one pass loads O (and J), finishes by the window's class (junction sums in chunk order, raw
+//            sums, windows without rows) and stores straight to the output: lane-consecutive streaming stores, 256 contiguous bytes
+//            per store instruction.  Nothing is written back to O.
 // Anything outside this fast path (irregular timestamps, DDV-long values, > 4 chunks, NaN / Inf / denormal / zero values, windows
 // shorter than 9 rows, windows over three chunks ...) is appended to the fallback list and answered by the v2 kernel into the same
 // output buffer, exactly as the tile kernel does.
@@ -37,9 +40,9 @@ __device__ __forceinline__ uint32_t wp_lds32(uint32_t off) { uint32_t v; asm vol
 #endif
 
 // Per-phase cycle counters of scan_wp_sum_kernel for profiling builds (-DFILO_WP_PROF; scratch/wp_prof.py): every lane reads the
-// SM clock at the phase boundaries of a series, lane 0 adds its sums to g_wp_prof (slots 0 .. 9: phases, 10 .. 13: event counts,
-// 15: warps).  32-bit sums (a warp's share of one launch is far below 2^32 cycles) keep the register cost low.  Compiled out of the
-// product build.
+// SM clock at the phase boundaries of a series, lane 0 adds its sums to g_wp_prof (slots 0 .. 9: phases, slot 8 empty since the finish
+// pass took over the result row; 10 .. 13: event counts, 15: warps).  32-bit sums (a warp's share of one launch is far below 2^32
+// cycles) keep the register cost low.  Compiled out of the product build.
 #if defined(FILO_WP_PROF) && !defined(FILO_CUSIM)
 __device__ unsigned long long g_wp_prof[16];
 #define WPROF_DECL uint32_t wpp_t0 = (uint32_t)clock(), wpp_acc[14] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
@@ -313,6 +316,32 @@ __device__ __forceinline__ uint32_t wp_decode(const uint8_t* R, double* V, const
   return okbits;
 }
 
+// Class of window k after the window blocks (chunks 0 .. n-1 of the plan in CD):
+//   WP_FINAL   the window block left the finished value in O;
+//   WP_RAWFIN  a raw sum in O: an own window of a block from tb on (that block stores raw sums because its later windows are shared);
+//   WP_JUNC    a raw sum at J[jslot & 127] (the chunk's blocks [0, jzb)); jslot & 128: the window is in the chunk's head share, and the
+//              earlier chunk's raw partial in O is added first (AggrOverTimeFunctions.scala:560-571);
+//   WP_GAP     no chunk has rows in the window: NaN (the reference leaves the NaN seed).
+constexpr uint32_t WP_FINAL = 0, WP_RAWFIN = 1, WP_JUNC = 2, WP_GAP = 3;
+__device__ __forceinline__ int wp_chunk_of(const WpChunk* CD, int n, int k) {      // the last chunk with blocks whose kT0 <= k, or -1
+  int ci = -1;
+  for (int c = 0; c < n; ++c) if (CD[c].nblk > 0 && k >= CD[c].kT0) ci = c;
+  return ci;
+}
+__device__ __forceinline__ uint32_t wp_class(const WpChunk* CD, int n, int k, uint32_t& jslot) {
+  const int ci = wp_chunk_of(CD, n, k);
+  jslot = 0;
+  if (ci < 0 || k > CD[ci].kT1) return WP_GAP;
+  const WpChunk& ch = CD[ci];
+  const int i = k - ch.kT0;
+  if (i < ch.jzb * WP_R) { jslot = (uint32_t)(ch.joff + i) | (i < ch.hs ? 128u : 0u); return WP_JUNC; }
+  return i >= ch.tb * WP_R ? WP_RAWFIN : WP_FINAL;       // (a window past ownHi belongs to the next chunk's head share)
+}
+__device__ __forceinline__ int wp_rows_in(const WpChunk& x, int k, int Wr) {    // rows of chunk x in window k
+  int lo = x.s0 + k; if (lo < 0) lo = 0; int hi = x.s0 + k + Wr; if (hi > x.nrows - 1) hi = x.nrows - 1;
+  return hi - lo + 1;
+}
+
 // window block `it` of the plan: V index of its first row, byte offset (inside the warp's region) of its first result slot, and
 // inf = (jEnd + 1) | raw << 4 | skew phase of the first slot << 5 | chunk << 8 | first window << 10, where slots 0 .. jEnd are stored
 __device__ __forceinline__ void wp_item(const WpChunk* CD, const WpSmem& L, int it, int items, int psi, int& pp, int& op, int& inf) {
@@ -370,7 +399,10 @@ scan_wp_sum_kernel(const uint8_t* __restrict__ arena, const int64_t* __restrict_
   // per-lane work items of the plan: two decode slots and the two window blocks of the first pass (see the plan)
   int dd_dst[2] = {0, 0}, dd_inf[2] = {0, 0}, wi_pp[2] = {0, 0}, wi_op[2] = {0, 0}, wi_inf[2] = {0, 0};
   int gz[3] = {-1, -1, -1}; bool gz_all = true;      // this lane's zero rows (V indices) when the plan has at most 96 of them
-  int p_Wr = 0, p_items = 0, p_nfull = 0, p_psi = 0; double p_rcpn = 0.0; bool p_gaps = true, p_oal = false;
+  int p_Wr = 0, p_items = 0, p_nfull = 0, p_psi = 0; double p_rcpn = 0.0; bool p_oal = false;
+  // classes of this lane's windows lane + 32 m, m < 16 (2 bits each, wp_class), and the J slots of its WP_JUNC windows among them in
+  // window order (8 bits each: at most 6, since the J slots of the plan are at most 128 over at most 3 chunks)
+  uint32_t p_cls = 0; uint64_t p_jx = 0;
   int64_t rows_scanned = 0, bytes_scanned = 0;
   uint32_t parity = 0;
 
@@ -434,16 +466,12 @@ scan_wp_sum_kernel(const uint8_t* __restrict__ arena, const int64_t* __restrict_
       const int jzb = (hs + WP_R - 1) / WP_R;
       const int tb = (touch && ownHi < kT1) ? (int)((ownHi + 1 - kT0) / WP_R) : nblk;
       if (touch && jzb > tb) okp = false;
-      int blk0, items, joff, jtot, cov;
+      int blk0, items, joff, jtot;
       { const int a0 = __shfl_sync(FULL, nblk, 0), a1 = __shfl_sync(FULL, nblk, 1), a2 = __shfl_sync(FULL, nblk, 2), a3 = __shfl_sync(FULL, nblk, 3);
         blk0 = (c > 0 ? a0 : 0) + (c > 1 ? a1 : 0) + (c > 2 ? a2 : 0); items = a0 + a1 + a2 + a3; }
       { const int z = jzb * WP_R;
         const int a0 = __shfl_sync(FULL, z, 0), a1 = __shfl_sync(FULL, z, 1), a2 = __shfl_sync(FULL, z, 2), a3 = __shfl_sync(FULL, z, 3);
         joff = (c > 0 ? a0 : 0) + (c > 1 ? a1 : 0) + (c > 2 ? a2 : 0); jtot = a0 + a1 + a2 + a3; }
-      { const int z = touch ? (int)(kT1 - kT0 + 1) - hs : 0;      // windows this chunk is the first to touch
-        cov = z;
-#pragma unroll
-        for (int o = 1; o < WP_MAXC; o <<= 1) cov += __shfl_xor_sync(FULL, cov, o); }
       if ((uint32_t)jtot > L.jcap) okp = false;
       if (L.alias && items > 64) okp = false;                 // O takes V's place: every block is summed before the first result is stored
       // row positions: chunk after chunk, Wr .. Wr + 7 zero rows in between, every chunk's block 0 at a multiple of 8
@@ -470,7 +498,6 @@ scan_wp_sum_kernel(const uint8_t* __restrict__ arena, const int64_t* __restrict_
           d.kT0 = (int)kT0; d.kT1 = (int)kT1; d.ownLo = (int)ownLo; d.ownHi = (int)ownHi; d.blk0 = blk0; d.nblk = nblk;
           d.vidx0 = wp_vidx(rowpos + fr); d.rowpos = rowpos; d.nrows = nrows; d.s0 = (int)s0; d.e0 = (int)e0; d.joff = joff; d.hs = hs; d.jzb = jzb; d.tb = tb;
         }
-        p_gaps = __shfl_sync(FULL, cov, 0) != q.T;
         // O is skewed like V (one pad slot per 8 windows, block starts of the first touched chunk on the 9-word grid): the 8-byte result
         // stores of a warp (lane stride 8 windows) then spread over the banks.  p_oal: every chunk's blocks start on that grid
         { const int first_t = tm ? __ffs((int)tm) - 1 : 0;
@@ -491,6 +518,18 @@ scan_wp_sum_kernel(const uint8_t* __restrict__ arena, const int64_t* __restrict_
             tot += g1 - g0;
           }
           gz_all = tot <= 96;
+        }
+        // window classes of the finish pass, for this lane's windows below T (windows from 512 on are classified in the pass itself)
+        {
+          uint32_t cls = 0; uint64_t jx = 0; int nj = 0;
+#pragma unroll 1
+          for (int m = 0; m < 16 && lane + 32 * m < q.T; ++m) {
+            uint32_t js;
+            const uint32_t code = wp_class(CD, n, lane + 32 * m, js);
+            cls |= code << (2 * m);
+            if (code == WP_JUNC) { jx |= (uint64_t)js << (8 * nj); ++nj; }
+          }
+          p_cls = cls; p_jx = jx;
         }
         // this lane's work items (they stay valid with the plan): decode slots lane, lane + 32 and window blocks lane, lane + 32
         {
@@ -624,58 +663,50 @@ scan_wp_sum_kernel(const uint8_t* __restrict__ arena, const int64_t* __restrict_
       }
       __syncwarp();
       WPROF(6)                                             // window blocks
-      // raw blocks: a window with rows from two chunks is (0 + partial of the earlier chunk) + partial of the later one
-      // (AggrOverTimeFunctions.scala:560-571); own windows that sit in a raw block are finished here as well
-      for (int ci = 0; ci < n; ++ci) {
-        const WpChunk& ch = CD[ci];
-        if (ch.jzb == 0 && ch.tb >= ch.nblk) continue;
-        auto rows_in = [&](const WpChunk& x, int k) -> int {
-          int lo = x.s0 + k; if (lo < 0) lo = 0; int hi = x.s0 + k + Wr; if (hi > x.nrows - 1) hi = x.nrows - 1;
-          return hi - lo + 1;
-        };
-        // head: blocks [0, jzb)
-        const int nh = ch.jzb * WP_R < ch.kT1 - ch.kT0 + 1 ? ch.jzb * WP_R : ch.kT1 - ch.kT0 + 1;
-        for (int i = lane; i < nh; i += 32) {
-          const int k = ch.kT0 + i;
-          double v = J[ch.joff + i]; int nn = 1;
-          if (FN == FN_AVG || FN == FN_COUNT) nn = rows_in(ch, k);
-          if (i < ch.hs) { v = O[oidx(k)] + v; if (FN == FN_AVG || FN == FN_COUNT) nn += rows_in(CD[ci - 1], k); }
-          O[oidx(k)] = wp_finish<FN>(v, nn, fdiv, frcp, 1000.0, p_nfull, p_rcpn, false);
-        }
-        // tail: own windows of block tb
-        for (int k = ch.kT0 + ch.tb * WP_R + lane; k <= ch.ownHi && ch.tb < ch.nblk; k += 32) {
-          int nn = 1;
-          if (FN == FN_AVG || FN == FN_COUNT) nn = rows_in(ch, k);
-          O[oidx(k)] = wp_finish<FN>(O[oidx(k)], nn, fdiv, frcp, 1000.0, p_nfull, p_rcpn, false);
-        }
-      }
-      // windows without rows: NaN (no chunk contributes: AggrOverTimeFunctions.scala:560-571 leaves the NaN seed)
-      if (p_gaps) {
-        int prev = -1;
-        for (int ci = 0; ci <= n; ++ci) {
-          int gend = q.T;
-          if (ci < n) { if (CD[ci].nblk == 0) continue; gend = CD[ci].kT0; }
-          for (int k = prev + 1 + lane; k < gend; k += 32) O[oidx(k)] = NaNv;
-          if (ci < n) prev = CD[ci].kT1;
-        }
-      }
-    }
-    // ------------------------------------------------------------------------------------------------ result row
-    __syncwarp();
-    WPROF(7)                                               // junction fix-up, gaps
-    {
+      // ---------------------------------------------------------------------------------------------- finish and store
       // lane-consecutive windows: 256 contiguous bytes per store instruction; O index of window lane + 32 m = oidx(lane) + 36 m
       double* gp = out + (size_t)s * q.T + lane;
       const double* sp = O + oidx(lane);
-      int iters = (q.T - lane + 31) >> 5;
-      for (; iters >= 4; iters -= 4, gp += 128, sp += 144) {
+      auto fin = [&](double o, uint32_t code, uint32_t js, int k) -> double {
+        double v = o;
+        if (code == WP_JUNC) { const double jv = J[js & 127u]; v = (js & 128u) ? o + jv : jv; }    // earlier chunk's partial first
+        double r;
+        if (FN == FN_COUNT) r = v;          // the raw blocks left (double) rows of their chunk: the junction sum is the window's count
+        else {
+          int nn = 1;
+          if (FN == FN_AVG && (code == WP_RAWFIN || code == WP_JUNC)) {
+            const int ci = wp_chunk_of(CD, n, k);
+            nn = wp_rows_in(CD[ci], k, Wr);
+            if (code == WP_JUNC && (js & 128u)) nn += wp_rows_in(CD[ci - 1], k, Wr);
+          }
+          r = wp_finish<FN>(v, nn, fdiv, frcp, 1000.0, p_nfull, p_rcpn, false);
+        }
+        return code == WP_FINAL ? o : code == WP_GAP ? NaNv : r;
+      };
+      uint32_t cls = p_cls; uint64_t jx = p_jx;
+      auto fin_m = [&](double o, int k) -> double {        // windows lane + 32 m, m < 16: class from the plan, J slot from the cursor
+        const uint32_t code = cls & 3u, js = (uint32_t)jx & 0xffu;
+        cls >>= 2;
+        if (code == WP_JUNC) jx >>= 8;
+        return fin(o, code, js, k);
+      };
+      int k = lane, iters = (q.T - lane + 31) >> 5;
+      int rest = iters > 16 ? iters - 16 : 0;
+      if (rest) iters = 16;
+      for (; iters >= 4; iters -= 4, gp += 128, sp += 144, k += 128) {
         const double v0 = sp[0], v1 = sp[36], v2 = sp[72], v3 = sp[108];
-        wp_store_result(gp, v0); wp_store_result(gp + 32, v1); wp_store_result(gp + 64, v2); wp_store_result(gp + 96, v3);
+        const double r0 = fin_m(v0, k), r1 = fin_m(v1, k + 32), r2 = fin_m(v2, k + 64), r3 = fin_m(v3, k + 96);
+        wp_store_result(gp, r0); wp_store_result(gp + 32, r1); wp_store_result(gp + 64, r2); wp_store_result(gp + 96, r3);
       }
-      for (; iters > 0; --iters, gp += 32, sp += 36) wp_store_result(gp, *sp);
+      for (; iters > 0; --iters, gp += 32, sp += 36, k += 32) wp_store_result(gp, fin_m(*sp, k));
+      for (; rest > 0; --rest, gp += 32, sp += 36, k += 32) {      // windows from 512 on (multi-pass plans only)
+        uint32_t js;
+        const uint32_t code = wp_class(CD, n, k, js);
+        wp_store_result(gp, fin(*sp, code, js, k));
+      }
     }
     __syncwarp();
-    WPROF(8)                                               // result row
+    WPROF(7)                                               // finish and store (slot 8, the former result row, stays empty)
   }
   WPROF(9)
   WPROF_FLUSH

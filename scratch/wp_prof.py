@@ -26,12 +26,17 @@ L.filo_debug_wp_prof(out.ctypes.data, 1)
 bench.main()
 L.filo_debug_wp_prof(out.ctypes.data, 0)
 names = ["wait: record (mbarrier)", "parse", "memo check (+ window plan on a miss)", "per-series descriptors, scan counters", "decode",
-         "zero rows", "window blocks", "junction fix-up, gaps", "result row", "loop head, declined series"]
+         "zero rows", "window blocks", "finish and store (earlier: fix-up, gaps)", None, "loop head, declined series"]
+# slot 8: the result row of builds before the finish pass took it over; empty since
 ns = float(out[10])
 tot = float(out[:10].sum())
 print("scan_wp_sum_kernel: %d warps, %d series taken up, %d memo misses, %d declined by the plan, %d declined by the values"
       % (int(out[15]), int(ns), int(out[11]), int(out[12]), int(out[13])))
 print("  %-40s %10s %7s" % ("phase", "cyc/series", "share"))
 for i, n in enumerate(names):
+    if n is None:
+        if out[i] == 0:
+            continue
+        n = "result row (earlier builds)"
     print("  %-40s %10.1f %6.1f %%" % (n, float(out[i]) / ns, 100.0 * float(out[i]) / tot))
 print("  %-40s %10.1f" % ("total", tot / ns))
