@@ -77,6 +77,7 @@ struct filo_table {
   int seg = 1;
   // histogram tables (value column = HistogramVector): one bucket scheme for the whole table
   bool hist = false, hist_exp = false; int hist_nb = 0;     // hist_exp: Base2ExpHistogramBuckets (histogram_quantile interpolates in log space)
+  bool hist_simple = false;                                  // some histogram vector is a simple (row) vector: not for the second scan kernel
   std::vector<double> hist_tops; double* d_hist_tops = nullptr;
 };
 
@@ -342,7 +343,7 @@ struct LoadIn { int64_t n_series; const int32_t* n_chunks; const uint64_t* addrs
                 GatherChunk* gc_out = nullptr; int64_t gc_base = 0; const std::vector<filo_ctx::HostRange>* ranges = nullptr;
                 int64_t cb0 = 0; };
 struct PlanTotals { int64_t chunks = 0, samples = 0, alg = 0; int32_t maxrows = 0, maxch = 0; uint32_t max_rec = 0, f_or = 0, f_and = ~0u;
-                    const uint8_t* hist_def = nullptr; bool any_scalar = false, hist_mismatch = false; bool all_in_ranges = true; };
+                    const uint8_t* hist_def = nullptr; bool any_scalar = false, hist_mismatch = false; bool all_in_ranges = true; bool hist_simple = false; };
 // same bucket scheme: format code, definition length and bytes of two HistogramVector headers (HistogramVector.matchBucketDef, :262-268)
 inline bool same_hist_def(const uint8_t* a, const uint8_t* b) {
   const int da = (uint16_t)(a[9] | (a[10] << 8)), db = (uint16_t)(b[9] | (b[10] << 8));
@@ -371,7 +372,7 @@ inline int plan_series(const LoadIn& in, int64_t i, SeriesPlan& out, PlanTotals&
     if (twire != WIRE_DDV_CONST) flags &= ~REC_ALL_TS_CONST;
     if (vv.drop) flags |= REC_ANY_DROP;
     if (vwire != WIRE_RAW64) flags |= REC_ANY_DECODE;
-    if (vv.hist) { flags |= REC_HIST; if (!tot.hist_def) tot.hist_def = vv.p; else if (vv.len > 0 && !same_hist_def(tot.hist_def, vv.p)) tot.hist_mismatch = true; }
+    if (vv.hist) { flags |= REC_HIST; if (vwire == WIRE_H_SIMPLE) tot.hist_simple = true; if (!tot.hist_def) tot.hist_def = vv.p; else if (vv.len > 0 && !same_hist_def(tot.hist_def, vv.p)) tot.hist_mismatch = true; }
     else tot.any_scalar = true;
     tot.samples += numRows; tot.alg += 28 + 16 + tv.total + vv.total;
     if (in.gc_out) {
@@ -395,7 +396,7 @@ inline void merge_totals(PlanTotals& a, const PlanTotals& b) {
   a.chunks += b.chunks; a.samples += b.samples; a.alg += b.alg; a.maxrows = std::max(a.maxrows, b.maxrows); a.maxch = std::max(a.maxch, b.maxch);
   a.max_rec = std::max(a.max_rec, b.max_rec); a.f_or |= b.f_or; a.f_and &= b.f_and;
   if (!a.hist_def) a.hist_def = b.hist_def; else if (b.hist_def && !same_hist_def(a.hist_def, b.hist_def)) a.hist_mismatch = true;
-  a.any_scalar |= b.any_scalar; a.hist_mismatch |= b.hist_mismatch; a.all_in_ranges = a.all_in_ranges && b.all_in_ranges;
+  a.any_scalar |= b.any_scalar; a.hist_mismatch |= b.hist_mismatch; a.hist_simple |= b.hist_simple; a.all_in_ranges = a.all_in_ranges && b.all_in_ranges;
 }
 // host NibblePack.unpackDoubleXOR (NibblePack.scala:374-447) for the custom bucket tops of a table (a few dozen values)
 inline bool host_unpack_double_xor(const uint8_t* buf, int cap, double* out, int n) {
@@ -583,6 +584,7 @@ static int32_t filo_load_series_impl(filo_ctx* ctx, int64_t n_series, const int3
   if (tot.hist_def) {                                  // histogram table: one bucket scheme, tops kept for histogram_quantile
     const int32_t rch = filo_internal_set_hist(ctx, t, tot.hist_def);
     if (rch != FILO_OK) { filo_table_free(ctx, t); return rch; }
+    t->hist_simple = tot.hist_simple;
   }
   // groups
   int32_t* d_gid = nullptr;
@@ -1452,14 +1454,14 @@ static int32_t filo_query_hist_impl(filo_ctx* ctx, const filo_table* t, int32_t 
   if (!ctx || !t || (!out_values && !out_quantile)) return fail(ctx, FILO_ERR_INVALID_ARG, "filo_query_hist: null argument");
   if (!t->hist) return fail(ctx, FILO_ERR_INVALID_ARG, "filo_query_hist: not a histogram table");
   if (agg != FILO_AGG_NONE && agg != FILO_AGG_SUM) return fail(ctx, FILO_ERR_UNSUPPORTED, "histogram aggregates: sum only");
-  if (!(fn == FILO_FN_RATE || fn == FILO_FN_INCREASE || fn == FILO_FN_SUM_OVER_TIME))
-    return fail(ctx, FILO_ERR_UNSUPPORTED, "histogram range functions on the device path: rate, increase, sum_over_time");
-  if (agg == FILO_AGG_NONE && out_quantile) return fail(ctx, FILO_ERR_INVALID_ARG, "histogram_quantile is applied to the aggregated histogram (aggr SUM)");
+  if (!(fn == FILO_FN_RATE || fn == FILO_FN_INCREASE || fn == FILO_FN_SUM_OVER_TIME || fn == FILO_FN_LAST))
+    return fail(ctx, FILO_ERR_UNSUPPORTED, "histogram range functions on the device path: rate, increase, sum_over_time, last");
   // PeriodicSamplesMapper.scala:45-49, 67-68
   if (start > end) return fail(ctx, FILO_ERR_INVALID_ARG, "start should be <= end");
   if (!(start == end || step > 0)) return fail(ctx, FILO_ERR_INVALID_ARG, "step should be > 0 for range query");
   if (start < end && step < ctx->cfg.min_step_ms) return fail(ctx, FILO_ERR_BAD_QUERY, "step should be at least min-step");
-  if (window <= 0) return fail(ctx, FILO_ERR_INVALID_ARG, "Need positive window lengths to apply range function");
+  const bool last = fn == FILO_FN_LAST;
+  if (window <= 0) { if (last) window = 5 * 60 * 1000 + 1; else return fail(ctx, FILO_ERR_INVALID_ARG, "Need positive window lengths to apply range function"); }
   CUDA_TRY(ctx, cudaSetDevice(ctx->device));
   cudaStream_t s = ctx->stream;
   const int64_t adjustedStep = step > 0 ? step : step + 1;
@@ -1468,8 +1470,18 @@ static int32_t filo_query_hist_impl(filo_ctx* ctx, const filo_table* t, int32_t 
   q.fn = fn; q.cumulative = (t->schema_flags & FILO_SCHEMA_CUMULATIVE) ? 1 : 0; q.inclusive = ctx->cfg.inclusive_range ? 1 : 0;
   const int nb = t->hist_nb, T = q.T;
   const bool fused = agg == FILO_AGG_SUM;
-  const size_t smem = hist_smem_bytes(t->max_rows, nb, T, fused, t->max_rec_bytes);
-  if (smem + 2048 > std::min<size_t>(ctx->max_smem_optin, 227 * 1024))
+  const bool pq = !fused && out_quantile;                // per-series histogram_quantile
+  const size_t smem = hist_smem_bytes(t->max_rows, nb, T, fused || pq, t->max_rec_bytes);
+  // second kernel: rate / increase over cumulative histograms and last over SectDelta vectors (its table parser takes no other vector),
+  // fused or per series, when its working set leaves room for two CTAs per SM
+  const size_t smem2 = hist2_smem_bytes(t->max_rows, nb, t->max_rec_bytes);
+  // Per series it takes the quantile and last; rate / increase bucket rows alone stay on the first kernel, whose (window, bucket) threads
+  // store [S][T][nb] contiguously (H100: 20.6 ms against 27.7 ms for 100 k series x 481 windows x 20 buckets, DESIGN §7).
+  const bool v2 = hist_v2_enabled() && ((q.cumulative && (fn == FILO_FN_RATE || fn == FILO_FN_INCREASE)) || (last && !t->hist_simple)) && T <= 32 * 512 && nb <= 64 &&
+                  smem2 + 1024 <= std::min<size_t>(ctx->max_smem_optin, 227 * 1024) && (fused || pq || last);
+  // the first kernel's working set (its per-series quantile and the fused sum keep a [T][nb] block in shared memory); a per-series query on
+  // the second kernel does not depend on it.  The fused sum keeps its limit whichever kernel runs it.
+  if (!(v2 && !fused) && smem + 2048 > std::min<size_t>(ctx->max_smem_optin, 227 * 1024))
     return fail(ctx, FILO_ERR_UNSUPPORTED, "histogram query does not fit the device working set (rows x buckets or windows x buckets too large)");
   Temp tmp(s);
   int* d_err = nullptr; unsigned long long* d_counters = nullptr;
@@ -1486,11 +1498,13 @@ static int32_t filo_query_hist_impl(filo_ctx* ctx, const filo_table* t, int32_t 
   if (out_values) CUDA_TRY(ctx, tmp.alloc((void**)&d_out, (size_t)rows * T * nb * 8));
   if (out_quantile) CUDA_TRY(ctx, tmp.alloc((void**)&d_q, (size_t)rows * T * 8));
   CUDA_TRY(ctx, cudaEventRecord(e0, s));
-  // second kernel: fused sum of rate / increase over cumulative histograms, when its working set leaves room for two CTAs per SM
-  const size_t smem2 = hist2_smem_bytes(t->max_rows, nb, t->max_rec_bytes);
-  const bool v2 = fused && hist_v2_enabled() && q.cumulative && (fn == FILO_FN_RATE || fn == FILO_FN_INCREASE) && T <= 32 * 512 && nb <= 64 &&
-                  smem2 + 1024 <= std::min<size_t>(ctx->max_smem_optin, 227 * 1024);
-  if (v2) {
+  if (v2 && !fused) {
+    const int cps = (int)std::max<size_t>(1, std::min<size_t>(2, (size_t)(228 * 1024) / (smem2 + 1024)));
+    L.grid = (int)std::max<int64_t>(1, std::min<int64_t>(hist2_series_items(t->n_series), (int64_t)ctx->sm_count * cps));
+    double* scratch = nullptr;                          // quantile only: each CTA's window columns, grid * T * nb doubles
+    if (!out_values) CUDA_TRY(ctx, tmp.alloc((void**)&scratch, (size_t)L.grid * T * nb * 8));
+    CUDA_TRY(ctx, launch_hist_scan2_series(L, nb, t->max_rows, t->max_rec_bytes, d_out, d_q, scratch, t->d_hist_tops, quantile, t->hist_exp ? 1 : 0));
+  } else if (v2) {
     const int cps = (int)std::max<size_t>(1, std::min<size_t>(2, (size_t)(228 * 1024) / (smem2 + 1024)));
     L.grid = (int)std::max<int64_t>(1, std::min<int64_t>(t->n_items, (int64_t)ctx->sm_count * cps));
     CUDA_TRY(ctx, tmp.alloc((void**)&pval, (size_t)t->n_items * T * nb * 8));
@@ -1503,7 +1517,7 @@ static int32_t filo_query_hist_impl(filo_ctx* ctx, const filo_table* t, int32_t 
     CUDA_TRY(ctx, launch_hist_scan(L, nb, t->max_rows, t->max_rec_bytes, t->grouped ? t->d_order : nullptr, t->d_item_begin, t->n_items, 1, nullptr, pval, pany));
     CUDA_TRY(ctx, launch_hist_merge(pval, pany, t->d_gis, t->n_groups, T, nb, t->hist_exp ? 1 : 0, t->d_hist_tops, out_quantile ? quantile : std::nan(""), d_out, d_q, s));
   } else {
-    CUDA_TRY(ctx, launch_hist_scan(L, nb, t->max_rows, t->max_rec_bytes, nullptr, nullptr, 0, 0, d_out, nullptr, nullptr));
+    CUDA_TRY(ctx, launch_hist_scan(L, nb, t->max_rows, t->max_rec_bytes, nullptr, nullptr, 0, 0, d_out, nullptr, nullptr, t->d_hist_tops, quantile, t->hist_exp ? 1 : 0, d_q));
   }
   CUDA_TRY(ctx, cudaEventRecord(e1, s));
   int herr[4]; unsigned long long hc[2];

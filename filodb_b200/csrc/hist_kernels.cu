@@ -116,9 +116,13 @@ __global__ void __launch_bounds__(HIST_THREADS)
 hist_scan_kernel(const uint8_t* __restrict__ arena, const int64_t* __restrict__ rec_off, int64_t n_series, QueryParams q, int nb, int max_rows, uint32_t max_rec,
                  const int32_t* __restrict__ order, const int64_t* __restrict__ item_begin, int64_t n_items, int agg,
                  double* __restrict__ out /* !agg: [S][T][nb] */, double* __restrict__ pval /* agg: [items][T][nb] */, uint8_t* __restrict__ pany,
-                 unsigned long long* d_counters, int* d_err) {
+                 unsigned long long* d_counters, int* d_err,
+                 const double* __restrict__ tops = nullptr, double qtl = 0.0, int exp_buckets = 0, double* __restrict__ out_q = nullptr /* !agg: [S][T] */) {
   extern __shared__ __align__(16) uint8_t smem[];
-  const HistLayout L = hist_layout(max_rows, nb, q.T, agg != 0, max_rec);
+  // per-series histogram_quantile (!agg, out_q given): each series' window rows are staged in acc[T][nb] (the fused mode's layout) and
+  // presented by a thread per window; out, when given, receives the staged rows
+  const bool pq = !agg && out_q != nullptr;
+  const HistLayout L = hist_layout(max_rows, nb, q.T, agg != 0 || pq, max_rec);
   int64_t* cv = reinterpret_cast<int64_t*>(smem + L.cv);
   int64_t* tss = reinterpret_cast<int64_t*>(smem + L.ts);
   int64_t* PT = reinterpret_cast<int64_t*>(smem + L.pt);
@@ -139,7 +143,8 @@ hist_scan_kernel(const uint8_t* __restrict__ arena, const int64_t* __restrict__ 
   int64_t rows_scanned = 0, bytes_scanned = 0;
   // sum mode: sum_over_time, and rate / increase on a delta-temporality schema (SumOverTimeChunkedFunctionH,
   // AggrOverTimeFunctions.scala:587-606; RateOverDeltaChunkedFunctionH, RateFunctions.scala:470-494)
-  const bool sum_mode = q.fn == FN_SUM || !q.cumulative;
+  const bool last = q.fn == FN_LAST;
+  const bool sum_mode = !last && (q.fn == FN_SUM || !q.cumulative);
   const double fdiv = (double)(q.inclusive ? winDur : winDur + 1), frcp = 1.0 / fdiv;       // windowEnd - curWindowStart
 
   HPROF_DECL
@@ -179,7 +184,7 @@ hist_scan_kernel(const uint8_t* __restrict__ arena, const int64_t* __restrict__ 
           const int defBytes = (int)(hv[9] | (hv[10] << 8));
           const int vnb = (int)(hv[11] | (hv[12] << 8));
           // counter functions need the SectDelta reader (a RowHistogramReader is not a CounterVectorReader, RangeFunction.scala:142)
-          if (!(wire == WIRE_H_SECTDELTA || (wire == WIRE_H_SIMPLE && sum_mode)) || vnb != nb || numHist < e.num_rows) { err = 1; break; }
+          if (!(wire == WIRE_H_SECTDELTA || (wire == WIRE_H_SIMPLE && (sum_mode || last))) || vnb != nb || numHist < e.num_rows) { err = 1; break; }
           HistChunkD d; d.sect = wire == WIRE_H_SECTDELTA; d.pad = 0; d.row_base = rows; d.nrows = e.num_rows; d.nsect = 0; d.has_drop = 0; d.end_time = e.end_time;
           const uint8_t* endp = hv + (int32_t)ld32(hv) + 4;
           const uint8_t* s = hv + 11 + defBytes; int start = 0;
@@ -226,6 +231,39 @@ hist_scan_kernel(const uint8_t* __restrict__ arena, const int64_t* __restrict__ 
       if (bad) { if (atomicCAS(&d_err[0], 0, 1) == 0) { d_err[1] = (int)(sid & 0x7fffffff); d_err[2] = (int)(sid >> 31); } }
       __syncthreads();
       HPROF(3)                                             // remaining rows decoded
+      // per-series histogram_quantile of the staged rows (Histogram.quantile, hist_quantile in hist_phases.h; empty windows: NaN)
+      auto present = [&]() {
+        for (int k = tid; k < q.T; k += HIST_THREADS)
+          out_q[(size_t)sid * q.T + k] = (any[k] && qtl == qtl) ? hist_quantile(acc + (size_t)k * nb, nb, tops, qtl, exp_buckets != 0) : NaNv;
+        if (out) for (int i = tid; i < q.T * nb; i += HIST_THREADS) out[(size_t)sid * q.T * nb + i] = acc[i];
+        __syncthreads();
+      };
+      if (last) {
+        // LastSampleChunkedFunctionH (RangeFunction.scala:599-641): over the window's chunk set, the row endRowNum = min(ceilingIndex(end),
+        // numRows - 1) of a chunk is kept when its timestamp is >= windowStart and > the one kept so far; the value is the raw reader value
+        // (SectDelta base + delta, or the row of a simple vector), without counter correction
+        for (int k = tid; k < q.T; k += HIST_THREADS) {
+          const int64_t wEnd = q.start + (int64_t)k * q.step;
+          const int row = hist_last_row(CH, n, tss, wEnd - winDur, wEnd);                // hist_phases.h, shared with the second kernel
+          const int64_t* rv = row >= 0 ? cv + (size_t)row * nb : nullptr;
+          if (!agg) {
+            double* o = pq ? acc + (size_t)k * nb : out + ((size_t)sid * q.T + k) * nb;
+            for (int b = 0; b < nb; ++b) o[b] = rv ? (double)rv[b] : NaNv;
+            if (pq) any[k] = rv != nullptr;
+          } else if (rv) {                                                    // HistSumRowAggregator: copy the first, MutableHistogram.add the others
+            const bool firstm = any[k] == 0; double mx = 0.0;
+            for (int b = 0; b < nb; ++b) {
+              double nv = acc[(size_t)k * nb + b] + (double)rv[b];
+              if (!firstm) { if (nv < mx || nv != nv) nv = mx; else if (nv > mx) mx = nv; }
+              acc[(size_t)k * nb + b] = nv;
+            }
+            any[k] = firstm ? 1 : 2;
+          }
+        }
+        __syncthreads();
+        if (pq) present();
+        continue;
+      }
       if (sum_mode) {
         // per-bucket running sums over the rows of each chunk (int64, exact): the reference adds the rows as doubles
         // (RowHistogramReader.sum, HistogramVector.scala:613-621), which is the same number while the sums stay below 2^53
@@ -262,7 +300,11 @@ hist_scan_kernel(const uint8_t* __restrict__ arena, const int64_t* __restrict__ 
             }
           }
           if (has && q.fn == FN_RATE) for (int b = 0; b < nb; ++b) hv[b] = hv[b] / (double)(wEnd - wStart) * 1000.0;   // RateFunctions.scala:481 (raw windowStart)
-          if (!agg) { double* o = out + ((size_t)sid * q.T + k) * nb; for (int b = 0; b < nb; ++b) o[b] = has ? hv[b] : NaNv; }
+          if (!agg) {
+            double* o = pq ? acc + (size_t)k * nb : out + ((size_t)sid * q.T + k) * nb;
+            for (int b = 0; b < nb; ++b) o[b] = has ? hv[b] : NaNv;
+            if (pq) any[k] = has;
+          }
           else if (has) {                                                     // HistSumRowAggregator: copy the first, MutableHistogram.add the others
             const bool firstm = any[k] == 0; double mx = 0.0;
             for (int b = 0; b < nb; ++b) {
@@ -274,6 +316,7 @@ hist_scan_kernel(const uint8_t* __restrict__ arena, const int64_t* __restrict__ 
           }
         }
         __syncthreads();
+        if (pq) present();
         continue;
       }
       // ---- corrections.  Inside a chunk (lazy val corrections, :690-707; correctedValue :730-746): every Drop section starting
@@ -352,6 +395,7 @@ hist_scan_kernel(const uint8_t* __restrict__ arena, const int64_t* __restrict__ 
           w.dTS = dTS; w.thr = thr; w.half = half; w.endpart = endpart; w.sI = sI; w.ratio0 = eTI / sI; w.skipC = 2.0 * dTS / sI;
         }
         W[k] = w;
+        if (pq) any[k] = w.hi_t > w.lo_t;
       }
       __syncthreads();
       HPROF(5)                                             // carried corrections + window descriptors
@@ -375,7 +419,8 @@ hist_scan_kernel(const uint8_t* __restrict__ arena, const int64_t* __restrict__ 
           r = q.fn == FN_RATE ? __dmul_rn(div_invariant(scaled, fdiv, frcp), 1000.0) : scaled;
           has = true;
         }
-        if (!agg) out[((size_t)sid * q.T + k) * nb + b] = r;                  // an empty histogram is returned as NaN buckets
+        if (pq) acc[i] = r;
+        else if (!agg) out[((size_t)sid * q.T + k) * nb + b] = r;             // an empty histogram is returned as NaN buckets
         else if (has) {                                                       // HistSumRowAggregator: empty histograms are skipped
           acc[i] += r;                                                        // (MutableHistogram.addNoCorrection: NaN-seeded sums start at 0)
           if (b == 0) any[k] = any[k] ? 2 : 1;                                // 1: the item's first histogram for this window (copied), 2: a further one
@@ -391,6 +436,7 @@ hist_scan_kernel(const uint8_t* __restrict__ arena, const int64_t* __restrict__ 
         }
         __syncthreads();
       }
+      if (pq) present();
       HPROF(6)                                             // (window, bucket) rates
     }
     if (agg) {
@@ -442,12 +488,12 @@ extern "C" int filo_debug_hist_prof(unsigned long long* out16, int reset) {
 
 size_t hist_smem_bytes(int max_rows, int nb, int T, bool agg, uint32_t max_rec) { return hist_layout(max_rows, nb, T, agg, max_rec).total; }
 cudaError_t launch_hist_scan(const ScanLaunch& L, int nb, int max_rows, uint32_t max_rec, const int32_t* order, const int64_t* item_begin, int64_t n_items, int agg,
-                             double* out, double* pval, uint8_t* pany) {
-  const size_t smem = hist_layout(max_rows, nb, L.q.T, agg != 0, max_rec).total;
+                             double* out, double* pval, uint8_t* pany, const double* tops, double qtl, int exp_buckets, double* out_q) {
+  const size_t smem = hist_layout(max_rows, nb, L.q.T, agg != 0 || (!agg && out_q), max_rec).total;
   cudaError_t e = cudaFuncSetAttribute(hist_scan_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess) return e;
   hist_scan_kernel<<<L.grid, HIST_THREADS, smem, L.stream>>>(L.arena, L.rec_off, L.n_series, L.q, nb, max_rows, max_rec, order, item_begin, n_items, agg,
-                                                             out, pval, pany, L.d_counters, L.d_err);
+                                                             out, pval, pany, L.d_counters, L.d_err, tops, qtl, exp_buckets, out_q);
   return cudaGetLastError();
 }
 cudaError_t launch_hist_merge(const double* pval, const uint8_t* pany, const int64_t* gis, int n_groups, int T, int nb, int exp_buckets, const double* tops, double q,

@@ -1,4 +1,5 @@
-// Histogram column scan, second version (fused sum of hist rate / increase over cumulative SectDelta histograms): the kernel that
+// Histogram column scan, second version (hist rate / increase over cumulative SectDelta histograms and hist last over SectDelta
+// histograms, fused sum or per series with histogram_quantile): the kernel that
 // strings the phases of hist_phases.h together.  filo_query_hist selects it for the shapes it serves (capi.cu; FILO_HIST_V2=0 turns it
 // off for A/B runs); the first version (hist_kernels.cu) serves every other shape.
 #include "kernels.h"
@@ -41,21 +42,34 @@ __device__ __forceinline__ void h2_stage_wait() { asm volatile("cp.async.wait_gr
 
 // One CTA folds work items (runs of series of one group, positions index `order`) into the item's partial row
 // pval[it][bucket][window] (bucket-major) and pany[it][window].
+// SERIES (per-series mode, no aggregate): a work item is the run of series [it * H2_RUN, ...), and the thread that owns a window presents the
+// series' own window histogram: its buckets to S.out_v[S][T][nb] and / or its Histogram.quantile to S.out_q[S][T].  Without out_v the buckets
+// pass through the CTA's column block S.scratch[cta][nb][T] (bucket-major: the owners of consecutive windows touch consecutive doubles), so
+// [S][T][nb] exists nowhere.  LAST: LastSampleChunkedFunctionH (h2_window_last); the counter corrections (P4-P6) do not run.
+constexpr int H2_RUN = 64;
+struct H2Series { double* out_v; double* out_q; double* scratch; const double* tops; double qtl; int exp_buckets; };
+template <bool SERIES = false, bool LAST = false>
 __global__ void __launch_bounds__(H2_THREADS, 2)
 hist_scan2_kernel(const uint8_t* __restrict__ arena, const int64_t* __restrict__ rec_off, QueryParams q, int nb, int max_rows, uint32_t max_rec,
                   const int32_t* __restrict__ order, const int64_t* __restrict__ item_begin, int64_t n_items,
-                  double* __restrict__ pval, uint8_t* __restrict__ pany, unsigned long long* d_counters, int* d_err) {
+                  double* __restrict__ pval, uint8_t* __restrict__ pany, unsigned long long* d_counters, int* d_err, H2Series S = H2Series{}, int64_t n_series = 0) {
   extern __shared__ __align__(16) uint8_t smem[];
   H2Ctx X; h2_ctx_init(X, smem, h2_layout(max_rows, nb, max_rec), q, nb);
   const int tid = threadIdx.x;
   int64_t rows_scanned = 0, bytes_scanned = 0;
   H2PROF_DECL
   for (int64_t it = blockIdx.x; it < n_items; it += gridDim.x) {
-    const int64_t pb = item_begin[it], pe = item_begin[it + 1];
-    double* pv = pval + (size_t)it * q.T * nb; uint8_t* pa = pany + (size_t)it * q.T;
-    for (int i = tid; i < q.T * nb; i += H2_THREADS) pv[i] = 0.0;
+    int64_t pb, pe;
+    double* pv = nullptr; uint8_t* pa = nullptr;
     uint32_t anyb = 0;                                   // bit j: window tid + j * H2_THREADS has a histogram
-    __syncthreads();                                     // the zero fill is visible to the owners of the windows
+    if constexpr (SERIES) {
+      pb = it * H2_RUN; pe = pb + H2_RUN < n_series ? pb + H2_RUN : n_series;
+    } else {
+      pb = item_begin[it]; pe = item_begin[it + 1];
+      pv = pval + (size_t)it * q.T * nb; pa = pany + (size_t)it * q.T;
+      for (int i = tid; i < q.T * nb; i += H2_THREADS) pv[i] = 0.0;
+      __syncthreads();                                   // the zero fill is visible to the owners of the windows
+    }
     bool prefetched = false;                             // the record of `pos` is already on its way (cp.async issued after the previous decode)
     for (int64_t pos = pb; pos < pe; ++pos) {
       const int64_t sid = order ? (int64_t)order[pos] : pos;
@@ -88,19 +102,34 @@ hist_scan2_kernel(const uint8_t* __restrict__ arena, const int64_t* __restrict__
       h2_add_base(tid, H2_THREADS, X);
       __syncthreads();
       H2PROF(3)                                           // next record issued, SectDelta bases added
-      h2_chunk_corrections(tid, H2_THREADS, X);
-      __syncthreads();
-      h2_chunk_less(tid, X);
-      __syncthreads();
-      h2_carried(tid, H2_THREADS, X);
-      __syncthreads();
+      if constexpr (!LAST) {
+        h2_chunk_corrections(tid, H2_THREADS, X);
+        __syncthreads();
+        h2_chunk_less(tid, X);
+        __syncthreads();
+        h2_carried(tid, H2_THREADS, X);
+        __syncthreads();
+      }
       H2PROF(4)                                           // corrections inside and across chunks
-      int j = 0;
-      for (int k = tid; k < q.T; k += H2_THREADS, ++j) if (h2_window(k, X, pv, !((anyb >> j) & 1u))) anyb |= 1u << j;
+      if constexpr (SERIES) {
+        const double NaNv = h2_nan();
+        for (int k = tid; k < q.T; k += H2_THREADS) {
+          // the window's buckets: in the output row when one is asked for (re-read below by this thread only), else in the CTA's column block
+          double* w = S.out_v ? S.out_v + ((size_t)sid * q.T + k) * nb : S.scratch + (size_t)blockIdx.x * q.T * nb + k;
+          const size_t ws = S.out_v ? 1 : (size_t)q.T;
+          const bool has = LAST ? h2_window_last<true>(k, X, w, true, ws) : h2_window<true>(k, X, w, true, ws);
+          if (!has && S.out_v) for (int b = 0; b < nb; ++b) w[b] = NaNv;                      // Histogram.empty: NaN buckets
+          if (S.out_q) S.out_q[(size_t)sid * q.T + k] = (has && S.qtl == S.qtl) ? hist_quantile(w, ws, nb, S.tops, S.qtl, S.exp_buckets != 0) : NaNv;
+        }
+      } else {
+        int j = 0;
+        if constexpr (LAST) { for (int k = tid; k < q.T; k += H2_THREADS, ++j) if (h2_window_last(k, X, pv, !((anyb >> j) & 1u))) anyb |= 1u << j; }
+        else { for (int k = tid; k < q.T; k += H2_THREADS, ++j) if (h2_window(k, X, pv, !((anyb >> j) & 1u))) anyb |= 1u << j; }
+      }
       __syncthreads();                                   // the series' rows and record are dead
       H2PROF(5)                                           // windows: descriptors + rates + partial-row update
     }
-    { int j = 0; for (int k = tid; k < q.T; k += H2_THREADS, ++j) pa[k] = (uint8_t)((anyb >> j) & 1u); }
+    if constexpr (!SERIES) { int j = 0; for (int k = tid; k < q.T; k += H2_THREADS, ++j) pa[k] = (uint8_t)((anyb >> j) & 1u); }
   }
   H2PROF_FLUSH
   if (tid == 0 && (rows_scanned | bytes_scanned)) { atomicAdd(&d_counters[0], (unsigned long long)rows_scanned); atomicAdd(&d_counters[1], (unsigned long long)bytes_scanned); }
@@ -140,13 +169,29 @@ extern "C" int filo_debug_hist2_prof(unsigned long long* out16, int reset) {
 }
 #endif
 size_t hist2_smem_bytes(int max_rows, int nb, uint32_t max_rec) { return h2_layout(max_rows, nb, max_rec).total; }
+template <bool SERIES, bool LAST>
+static cudaError_t launch_hist_scan2_t(const ScanLaunch& L, int nb, int max_rows, uint32_t max_rec, const int32_t* order, const int64_t* item_begin, int64_t n_items,
+                                       double* pval, uint8_t* pany, const H2Series& S) {
+  const size_t smem = h2_layout(max_rows, nb, max_rec).total;
+  cudaError_t e = cudaFuncSetAttribute(hist_scan2_kernel<SERIES, LAST>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  if (e != cudaSuccess) return e;
+  hist_scan2_kernel<SERIES, LAST><<<L.grid, H2_THREADS, smem, L.stream>>>(L.arena, L.rec_off, L.q, nb, max_rows, max_rec, order, item_begin, n_items, pval, pany,
+                                                                          L.d_counters, L.d_err, S, L.n_series);
+  return cudaGetLastError();
+}
 cudaError_t launch_hist_scan2(const ScanLaunch& L, int nb, int max_rows, uint32_t max_rec, const int32_t* order, const int64_t* item_begin, int64_t n_items,
                               double* pval, uint8_t* pany) {
-  const size_t smem = h2_layout(max_rows, nb, max_rec).total;
-  cudaError_t e = cudaFuncSetAttribute(hist_scan2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-  if (e != cudaSuccess) return e;
-  hist_scan2_kernel<<<L.grid, H2_THREADS, smem, L.stream>>>(L.arena, L.rec_off, L.q, nb, max_rows, max_rec, order, item_begin, n_items, pval, pany, L.d_counters, L.d_err);
-  return cudaGetLastError();
+  const H2Series S{};
+  return L.q.fn == FN_LAST ? launch_hist_scan2_t<false, true>(L, nb, max_rows, max_rec, order, item_begin, n_items, pval, pany, S)
+                           : launch_hist_scan2_t<false, false>(L, nb, max_rows, max_rec, order, item_begin, n_items, pval, pany, S);
+}
+int64_t hist2_series_items(int64_t n_series) { return (n_series + H2_RUN - 1) / H2_RUN; }
+cudaError_t launch_hist_scan2_series(const ScanLaunch& L, int nb, int max_rows, uint32_t max_rec, double* out_values, double* out_q, double* scratch,
+                                     const double* tops, double qtl, int exp_buckets) {
+  const H2Series S{out_values, out_q, scratch, tops, qtl, exp_buckets};
+  const int64_t n_items = hist2_series_items(L.n_series);
+  return L.q.fn == FN_LAST ? launch_hist_scan2_t<true, true>(L, nb, max_rows, max_rec, nullptr, nullptr, n_items, nullptr, nullptr, S)
+                           : launch_hist_scan2_t<true, false>(L, nb, max_rows, max_rec, nullptr, nullptr, n_items, nullptr, nullptr, S);
 }
 cudaError_t launch_hist_merge2(const double* pval, const uint8_t* pany, const int64_t* gis, int n_groups, int T, int nb, int exp_buckets, const double* tops, double q,
                                double* out_values, double* out_q, cudaStream_t s) {

@@ -342,7 +342,9 @@ inline double h2_clamped_ratio(double sI, double lo, double delta, double dTS, d
 // P7 (thread per window): chunk set, row ranges, lowest / highest sample (HistogramRateFunctionBase.addTimeChunks, RateFunctions.scala:349-364),
 // then extrapolatedRate per bucket (:72-111, :366-407) folded into the item's partial row pv[b * T + k] (HistSumRowAggregator: empty
 // histograms are skipped; `first`: no series of the item has produced a histogram for this window yet).  Returns true when the window produced a histogram.
-FILO_HD inline bool h2_window(int k, const H2Ctx& X, double* pv, bool first) {
+// SERIES: the series' own window histogram is stored, bucket b at pv[b * ws] (pv already points at the window's first bucket).
+template <bool SERIES = false>
+FILO_HD inline bool h2_window(int k, const H2Ctx& X, double* pv, bool first, size_t ws = 0) {
   const H2Ctl* C = X.ctl(); const int64_t* cv = X.cv(); const int64_t* tss = X.ts(); const int64_t* PT = X.PT();
   const QueryParams& q = X.q; const int n = C->n, nb = X.nb, pitch = X.L.pitch;
   const int64_t wEnd = q.start + (int64_t)k * q.step, wStart = wEnd - X.winDur;
@@ -394,12 +396,12 @@ FILO_HD inline bool h2_window(int k, const H2Ctx& X, double* pv, bool first) {
   // HistSumRowAggregator.reduceAggregate (HistSumRowAggregator.scala:25-36): the first histogram of the partial row is copied, every
   // further one goes through MutableHistogram.add = addNoCorrection + makeMonotonic (Histogram.scala:428-449): running maximum mx
   double mx = 0.0;
-  double* pk = pv + k;                                                      // bucket b of window k at pk[b * T]
-  const size_t Tq = (size_t)q.T;
+  double* pk = SERIES ? pv : pv + k;                                        // bucket b of window k at pk[b * T] (SERIES: pk[b * ws])
+  const size_t Tq = SERIES ? ws : (size_t)q.T;
   for (int b0 = 0; b0 < nb; b0 += H2_BATCH, pk += (size_t)H2_BATCH * Tq) {
     double old[H2_BATCH];
 #pragma unroll
-    for (int j = 0; j < H2_BATCH; ++j) if (b0 + j < nb) old[j] = pk[(size_t)j * Tq];
+    for (int j = 0; j < H2_BATCH; ++j) if (!SERIES && b0 + j < nb) old[j] = pk[(size_t)j * Tq];
 #pragma unroll
     for (int j = 0; j < H2_BATCH; ++j) {
       const int b = b0 + j;
@@ -413,6 +415,7 @@ FILO_HD inline bool h2_window(int k, const H2Ctx& X, double* pv, bool first) {
           ratio = h2_clamped_ratio(sI, lo, delta, dTS, thr, half, endpart);
         const double scaled = delta * ratio;
         const double r = is_rate ? h2_div_window(scaled, X.fdiv, X.frcp) * 1000.0 : scaled;
+        if (SERIES) { pk[(size_t)j * Tq] = r; continue; }
         double nv = old[j] + r;                                             // MutableHistogram.addNoCorrection: NaN-seeded sums start at 0
         if (!first) { nv = nv >= mx ? nv : mx; mx = nv > mx ? nv : mx; }    // makeMonotonic: below the running maximum (or NaN) -> the maximum
         pk[(size_t)j * Tq] = nv;
@@ -422,26 +425,75 @@ FILO_HD inline bool h2_window(int k, const H2Ctx& X, double* pv, bool first) {
   return true;
 }
 
-// Histogram.quantile (vectors/Histogram.scala:65-108; min = 0, max = +Inf, evenDistribution = false) over cumulative bucket sums v[nb] with
-// bucket tops tops[nb]; exp_buckets: Base2ExpHistogramBuckets interpolate in log2 space except in the zero bucket (:97-104, log2 :111)
-FILO_HD inline double hist_quantile(const double* v, int nb, const double* tops, double qtl, bool exp_buckets) {
+// `last` of one window, shared by both histogram kernels (ch: their chunk descriptors with row_base / nrows / end_time, tss: the decoded
+// timestamps of the series' rows): LastSampleChunkedFunction.addChunks (RangeFunction.scala:599-614) keeps, over the window's chunk set
+// (as h2_window), the row endRowNum = min(ceilingIndex(windowEnd), numRows - 1) of a chunk when its timestamp is >= windowStart and > the
+// timestamp kept so far.  Returns that row, or -1 (Histogram.empty).
+template <class Chunk>
+FILO_HD inline int hist_last_row(const Chunk* ch, int n, const int64_t* tss, int64_t wStart, int64_t wEnd) {
+  int64_t kept = -1; int row = -1;                                      // LastSampleChunkedFunction.timestamp starts at -1
+  for (int c = 0; c < n; ++c) {
+    const Chunk& d = ch[c];
+    if (d.end_time < wStart) continue;                                  // ChunkSetInfo.scala:481-510 (time-ordered chunks)
+    if (c > 0 && !(ch[c - 1].end_time < wEnd)) continue;
+    const int64_t* t = tss + d.row_base;
+    int lo = 0, hi = d.nrows;                                           // ceilingIndex: rows with ts <= wEnd, minus one
+    while (lo < hi) { const int m = (lo + hi) >> 1; if (t[m] <= wEnd) lo = m + 1; else hi = m; }
+    int e = lo - 1; if (e > d.nrows - 1) e = d.nrows - 1;
+    if (e >= 0 && t[e] >= wStart && t[e] > kept) { kept = t[e]; row = d.row_base + e; }
+  }
+  return row;
+}
+// P7 for `last` (thread per window; P4-P6 do not run, the rows hold the raw reader values after P3)
+FILO_HD inline int h2_last_row(int k, const H2Ctx& X) {
+  const int64_t wEnd = X.q.start + (int64_t)k * X.q.step;
+  return hist_last_row(X.ctl()->ch, X.ctl()->n, X.ts(), wEnd - X.winDur, wEnd);
+}
+// `last` of window k: LastSampleChunkedFunctionH.updateValue takes asHistReader(endRowNum), the raw value (no counter correction).
+// Fused: folded into the partial row like h2_window; SERIES: stored at pv[b * ws].
+template <bool SERIES = false>
+FILO_HD inline bool h2_window_last(int k, const H2Ctx& X, double* pv, bool first, size_t ws = 0) {
+  const int row = h2_last_row(k, X);
+  if (row < 0) return false;
+  const int64_t* r = X.cv() + (size_t)row * X.L.pitch;
+  const int nb = X.nb;
+  double* pk = SERIES ? pv : pv + k;
+  const size_t Tq = SERIES ? ws : (size_t)X.q.T;
+  double mx = 0.0;
+  for (int b = 0; b < nb; ++b) {
+    const double v = (double)r[b];
+    if (SERIES) { pk[(size_t)b * Tq] = v; continue; }
+    double nv = pk[(size_t)b * Tq] + v;                                 // HistSumRowAggregator fold, as in h2_window
+    if (!first) { nv = nv >= mx ? nv : mx; mx = nv > mx ? nv : mx; }
+    pk[(size_t)b * Tq] = nv;
+  }
+  return true;
+}
+
+// Histogram.quantile (vectors/Histogram.scala:65-108; min = 0, max = +Inf, evenDistribution = false) over cumulative bucket sums v[b * vs]
+// with bucket tops tops[nb]; exp_buckets: Base2ExpHistogramBuckets interpolate in log2 space except in the zero bucket (:97-104, log2 :111).
+// No makeMonotonic: firstBucketGTE walks up from bucket 0 as the reference does, also over a non-monotonic per-series histogram.
+FILO_HD inline double hist_quantile(const double* v, size_t vs, int nb, const double* tops, double qtl, bool exp_buckets) {
   const double NaNv = h2_nan(), Inf = HUGE_VAL;
-  const double top = v[nb - 1];
+  const double top = v[(size_t)(nb - 1) * vs];
   if (qtl < 0) return -Inf;
   if (qtl > 1) return Inf;
   if (nb < 2 || !(top > 0)) return NaNv;
   double rank = qtl * top;
-  int bucket = 0; while (v[bucket] < rank) ++bucket;
+  int bucket = 0; while (v[(size_t)bucket * vs] < rank) ++bucket;
   const double bucketStart = bucket == 0 ? 0.0 : tops[bucket - 1];
   const double bucketEnd = tops[bucket];
   if (bucket == nb - 1 && bucketEnd == Inf) return tops[nb - 2];
   if (bucket == 0 && tops[0] <= 0) return tops[0];
-  const double count = bucket == 0 ? v[bucket] : v[bucket] - v[bucket - 1];
-  rank -= (bucket == 0 ? 0.0 : v[bucket - 1]);
+  const double count = bucket == 0 ? v[(size_t)bucket * vs] : v[(size_t)bucket * vs] - v[(size_t)(bucket - 1) * vs];
+  rank -= (bucket == 0 ? 0.0 : v[(size_t)(bucket - 1) * vs]);
   const double fraction = rank / count;
   if (!exp_buckets || bucketStart == 0) return bucketStart + (bucketEnd - bucketStart) * fraction;
   const double ln2 = log(2.0), logEnd = log(bucketEnd) / ln2, logStart = log(bucketStart) / ln2;
   return pow(2.0, logStart + (logEnd - logStart) * fraction);
+}
+FILO_HD inline double hist_quantile(const double* v, int nb, const double* tops, double qtl, bool exp_buckets) {
+  return hist_quantile(v, (size_t)1, nb, tops, qtl, exp_buckets);
 }
 
 } // namespace filo

@@ -58,14 +58,20 @@ cudaError_t launch_scan_wp_ctr(const ScanLaunch& L, double* out, const WpCtrSmem
 cudaError_t launch_scan_wp_ctr_agg(const ScanLaunch& L, const WpCtrSmem& W, const int32_t* order, const int64_t* item_begin, int64_t n_items, int agg_op,
                                    double* pval, uint32_t* pcnt, int64_t* fallback_list, unsigned long long* fallback_count, bool moments = false);
 size_t hist_smem_bytes(int max_rows, int nb, int T, bool agg, uint32_t max_rec);
+// agg == 0 with out_q: per-series histogram_quantile (tops, qtl, exp_buckets) to out_q [S][T], the rows to out when given
 cudaError_t launch_hist_scan(const ScanLaunch& L, int nb, int max_rows, uint32_t max_rec, const int32_t* order, const int64_t* item_begin, int64_t n_items, int agg,
-                             double* out, double* pval, uint8_t* pany);
+                             double* out, double* pval, uint8_t* pany, const double* tops = nullptr, double qtl = 0.0, int exp_buckets = 0, double* out_q = nullptr);
 cudaError_t launch_hist_merge(const double* pval, const uint8_t* pany, const int64_t* gis, int n_groups, int T, int nb, int exp_buckets, const double* tops, double q,
                               double* out_values, double* out_q, cudaStream_t s);
-// second version of the histogram scan (hist_kernels2.cu): fused sum of rate / increase over cumulative SectDelta histograms
+// second version of the histogram scan (hist_kernels2.cu): rate / increase over cumulative SectDelta histograms and last over SectDelta
+// histograms, fused sum (launch_hist_scan2) or per series (launch_hist_scan2_series: buckets to out_values [S][T][nb] and / or
+// histogram_quantile to out_q [S][T]; without out_values, scratch holds grid * T * nb doubles)
 size_t hist2_smem_bytes(int max_rows, int nb, uint32_t max_rec);
 cudaError_t launch_hist_scan2(const ScanLaunch& L, int nb, int max_rows, uint32_t max_rec, const int32_t* order, const int64_t* item_begin, int64_t n_items,
                               double* pval, uint8_t* pany);
+int64_t hist2_series_items(int64_t n_series);
+cudaError_t launch_hist_scan2_series(const ScanLaunch& L, int nb, int max_rows, uint32_t max_rec, double* out_values, double* out_q, double* scratch,
+                                     const double* tops, double qtl, int exp_buckets);
 cudaError_t launch_hist_merge2(const double* pval, const uint8_t* pany, const int64_t* gis, int n_groups, int T, int nb, int exp_buckets, const double* tops, double q,
                                double* out_values, double* out_q, cudaStream_t s);
 cudaError_t launch_iota(int32_t* a, int64_t n, cudaStream_t s);

@@ -115,9 +115,9 @@ class FusedGpuExec:
                     if aggr and aggr.aggrOp != capi.AGG_SUM:
                         raise capi.FiloError(capi.ERR_UNSUPPORTED, "histogram aggregates: sum only")
                     res = self.ctx.query_hist(tab, fn, psm.startMs, psm.stepMs, psm.endMs, window, aggr=capi.AGG_SUM if aggr else capi.AGG_NONE,
-                                              quantile=quantile.q if quantile else None)
-                    vals, q = res if isinstance(res, tuple) else (res, None)
-                    return QueryResult(q if quantile else vals, None, dict(self.ctx.last_stats))
+                                              quantile=quantile.q if quantile else None, want_values=quantile is None)
+                    # [rows, T, buckets], or with the quantile [rows, T]; rows = groups, or series without an aggregate
+                    return QueryResult(res, None, dict(self.ctx.last_stats))
                 k = int(aggr.aggrParams[0]) if aggr.aggrOp in (capi.AGG_TOPK, capi.AGG_BOTTOMK) else 0
                 res = self.ctx.query(tab, fn, psm.startMs, psm.stepMs, psm.endMs, window, aggr=aggr.aggrOp, k=k)
                 vals, aux = res if isinstance(res, tuple) else (res, None)

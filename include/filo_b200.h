@@ -258,10 +258,15 @@ int32_t filo_query_avg_sum_count(filo_ctx* ctx, const filo_table* t_sum, const f
  * ExpHistogramVector columns (wire 0x1309, a scheme per row) and the XOR-packed codes 0x08 / 0x0a / 0x10 are declined with
  * FILO_ERR_UNSUPPORTED; filo_table_info.schema_flags keeps the caller's flags.  filo_query_hist runs
  *   HistRateFunction / HistIncreaseFunction (RateFunctions.scala:330-418) over cumulative SectDelta histograms with counter
- *   correction (SectDeltaHistogramReader, HistogramVector.scala:628-738), optionally HistSumRowAggregator
- *   (aggregator/HistSumRowAggregator.scala) over the table's groups and HistogramQuantileImpl (InstantFunction.scala:362-368).
- *  aggr NONE: out_values [n_series * T * buckets] (an empty histogram = NaN buckets), out_quantile must be NULL
+ *   correction (SectDeltaHistogramReader, HistogramVector.scala:628-738), sum_over_time (and rate / increase over a delta-temporality
+ *   schema), or LastSampleChunkedFunctionH (range_fn FILO_FN_LAST, RangeFunction.scala:595-641: per window the latest row of the
+ *   window's chunks, the raw reader value without counter correction; window_ms <= 0 takes the 5 min + 1 ms default lookback),
+ *   optionally HistSumRowAggregator (aggregator/HistSumRowAggregator.scala) over the table's groups, and HistogramQuantileImpl
+ *   (InstantFunction.scala:362-368).
+ *  aggr NONE: out_values [n_series * T * buckets] (an empty histogram = NaN buckets) or NULL, out_quantile [n_series * T] or NULL:
+ *             the quantile of each series' own window histogram (Histogram.quantile, no makeMonotonic), NaN for an empty one
  *  aggr SUM : out_values [n_groups * T * buckets] or NULL, out_quantile [n_groups * T] or NULL (quantile in [0,1])
+ *  At least one of the two outputs is given; a quantile < 0 gives -Inf, > 1 gives +Inf (for a non-empty histogram).
  * The sum follows HistSumRowAggregator.reduceAggregate (HistSumRowAggregator.scala:25-36): the first histogram of a partial aggregate
  * is copied, every further one goes through MutableHistogram.add = addNoCorrection + makeMonotonic (Histogram.scala:428-449).  That
  * holds inside a work item (a run of series of one group, in series order) and across the items of a group (item order) -- the

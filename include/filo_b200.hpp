@@ -134,9 +134,9 @@ class FusedGpuExec {
       filo_table_info ti{}; filo_table_get_info(t, &ti);
       r.rows = aggr ? nGroups : (int32_t)source.size();
       if (aggr && aggr->aggrOp != AggregationOperator::Sum) throw QueryError(FILO_ERR_UNSUPPORTED, "histogram aggregates: sum only");
-      if (quantile) {
+      if (quantile) {                             // [rows][T]: the quantile of each group's sum, or of each series' own histogram
         r.values.assign((size_t)r.rows * r.windows, 0.0);
-        check(filo_query_hist(ctx_, t, fn, psm.startMs, psm.stepMs, psm.endMs, window, FILO_AGG_SUM, quantile->q, nullptr, r.values.data(), &r.stats));
+        check(filo_query_hist(ctx_, t, fn, psm.startMs, psm.stepMs, psm.endMs, window, aggr ? FILO_AGG_SUM : FILO_AGG_NONE, quantile->q, nullptr, r.values.data(), &r.stats));
       } else {
         r.buckets = ti.hist_buckets; r.values.assign((size_t)r.rows * r.windows * r.buckets, 0.0);
         check(filo_query_hist(ctx_, t, fn, psm.startMs, psm.stepMs, psm.endMs, window, aggr ? FILO_AGG_SUM : FILO_AGG_NONE, std::nan(""), r.values.data(), nullptr, &r.stats));
