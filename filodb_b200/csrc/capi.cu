@@ -920,6 +920,9 @@ static int32_t query_device_impl(filo_ctx* ctx, const filo_table* t, int32_t fn,
     const bool alias = wp_max_items((uint32_t)t->max_chunks, (uint32_t)q.T, (uint32_t)wrows) <= 64;
     WL = wp_layout(t->max_rec_bytes, (uint32_t)t->max_rows, (uint32_t)t->max_chunks, (uint32_t)q.T, (uint32_t)wrows, alias);
     WL.warps = (uint32_t)std::min<size_t>(smem_cap / WL.per_warp, alias ? WP_MAX_WARPS_ALIAS : WP_MAX_WARPS);
+    // two record buffers per warp (the records of the next two series in flight) when 16 warps of them fit
+    const WpSmem WL2 = wp_layout(t->max_rec_bytes, (uint32_t)t->max_rows, (uint32_t)t->max_chunks, (uint32_t)q.T, (uint32_t)wrows, alias, true);
+    if (smem_cap / WL2.per_warp >= (size_t)WP_MAX_WARPS) { WL = WL2; WL.warps = WP_MAX_WARPS; }
     use_wp = WL.warps >= 4;
   }
   // v4 counter-class kernel (scan_wp_ctr.cuh): per-series rows, or fused partial rows of up to TILE_AGG_ACC * TILE_THREADS windows;

@@ -3,7 +3,8 @@
 // Each warp runs its own three-buffer pipeline in shared memory:
 //   R  the series' record (ChunkSetInfo entries + BinaryVectors verbatim), filled by ONE cp.async.bulk (TMA 1-D) per series that is
 //      issued as soon as the previous record is no longer read (its fields extracted, raw f64 vectors copied), i.e. it is in flight
-//      during the rest of the previous series' decode and its window phase;
+//      during the rest of the previous series' decode and its window phase.  With two record buffers (L.rec2) the warp's series
+//      alternate between them, and the copy issued there is the record of the series after next: two records are in flight;
 //   V  the decoded rows, laid out per chunk with zero rows in between so that clamped windows read +0.0 instead of testing bounds
 //      (x + 0.0 == x for every sum of non-zero values and +0.0 rows), skewed by one pad slot per 8 rows: both the 8-byte row stores of the
 //      group decode (lane stride 8 rows) and the 8-byte row loads of the window blocks (lane stride 8 windows) then walk the banks with
@@ -379,12 +380,14 @@ scan_wp_sum_kernel(const uint8_t* __restrict__ arena, const int64_t* __restrict_
   WpChunk* CD = reinterpret_cast<WpChunk*>(wb + WP_OFF_DESC);
   uint64_t* xtab = reinterpret_cast<uint64_t*>(wb + WP_OFF_J);     // decode: exclusive XOR prefix per group slot (dead before J is written)
   double* J = reinterpret_cast<double*>(wb + WP_OFF_J);
+  // R: this series' record; with two record buffers the warp's series alternate between them (stage = iteration & 1)
+  const bool two = L.rec2 != 0;
   uint8_t* R = wb + WP_OFF_REC;
   double* V = reinterpret_cast<double*>(wb + L.vals);
   double* O = reinterpret_cast<double*>(wb + L.out);
   const int64_t nwarps = (int64_t)gridDim.x * (blockDim.x >> 5);
   int64_t s = (int64_t)blockIdx.x * (blockDim.x >> 5) + warp;
-  if (lane == 0) { mbar_init(bar, 1); mbar_fence_init(); }
+  if (lane == 0) { mbar_init(bar, 1); if (two) mbar_init(bar + 1, 1); mbar_fence_init(); }
   __syncwarp();
 
   int64_t winDur = q.inclusive ? q.window : q.window - 1; if (winDur < 0) winDur = 0;
@@ -406,24 +409,35 @@ scan_wp_sum_kernel(const uint8_t* __restrict__ arena, const int64_t* __restrict_
   int64_t rows_scanned = 0, bytes_scanned = 0;
   uint32_t parity = 0;
 
-  auto issue = [&](int64_t off, uint32_t sz) {            // lane 0: fetch a record into R
-    mbar_expect_tx(bar, sz);
-    tma_load_1d(R, arena + off, sz, bar);
+  auto issue = [&](int64_t off, uint32_t sz) {            // lane 0: fetch a record into R (the buffer of the current stage)
+    uint64_t* b = bar + (R == wb + WP_OFF_REC ? 0 : 1);
+    mbar_expect_tx(b, sz);
+    tma_load_1d(R, arena + off, sz, b);
   };
-  int64_t cur_off = 0; uint32_t cur_sz = 0;
+  // cur_sz: size of the record of series s; with two buffers, nb_sz: of series s + nwarps (already in flight in the other buffer)
+  uint32_t cur_sz = 0, nb_sz = 0;
+  int64_t cur_off = 0;
   if (s < n_series) { cur_off = rec_off[s]; cur_sz = (uint32_t)(rec_off[s + 1] - cur_off); }
   if (s < n_series && cur_sz <= L.rec_cap && lane == 0) issue(cur_off, cur_sz);
+  if (two && s + nwarps < n_series) {
+    const int64_t o1 = rec_off[s + nwarps]; nb_sz = (uint32_t)(rec_off[s + nwarps + 1] - o1);
+    R = wb + L.rec2;
+    if (nb_sz <= L.rec_cap && lane == 0) issue(o1, nb_sz);
+    R = wb + WP_OFF_REC;
+  }
+  uint32_t stage = 0;
   WPROF_DECL
 
   for (; s < n_series; s += nwarps) {
-    const int64_t sn = s + nwarps;
-    // the next record's offsets: loaded here, their difference taken after the parse, so that the loads' latency passes behind it
+    // the record this iteration issues: series s + nwarps (one buffer) or s + 2 nwarps (two buffers), into this series' buffer
+    const int64_t sn = s + (two ? 2 : 1) * nwarps;
+    // its offsets: loaded here, their difference taken after the parse, so that the loads' latency passes behind it
     int64_t nxt_off = 0; uint32_t nxt_end = 0;                 // (the size needs the low word of the end only)
     if (sn < n_series) { nxt_off = rec_off[sn]; nxt_end = (uint32_t)rec_off[sn + 1]; }
     const bool staged = cur_sz <= L.rec_cap;
     WPROF_COUNT(10)
     WPROF(9)                                               // loop head (+ the declined series' exits)
-    if (staged) { mbar_wait(bar, parity); parity ^= 1; }
+    if (staged) { mbar_wait(bar + stage, (parity >> stage) & 1u); parity ^= 1u << stage; }      // bit b: phase of buffer b's mbarrier
     WPROF(0)                                               // wait: record
     // ------------------------------------------------------------------------------------------------ setup (lane c = chunk c)
     const WpParsed P = wp_parse<true>(R, q, staged, lane);
@@ -559,7 +573,7 @@ scan_wp_sum_kernel(const uint8_t* __restrict__ arena, const int64_t* __restrict_
       if (lane == 0) { const unsigned long long slot = atomicAdd(fallback_count, 1ull); fallback_list[slot] = s; }
       __syncwarp();
       if (sn < n_series && nxt_sz <= L.rec_cap && lane == 0) issue(nxt_off, nxt_sz);
-      cur_off = nxt_off; cur_sz = nxt_sz;
+      if (two) { cur_sz = nb_sz; nb_sz = nxt_sz; stage ^= 1u; R = wb + (stage ? L.rec2 : WP_OFF_REC); } else cur_sz = nxt_sz;
       continue;
     }
     // per-series parts of the descriptors
@@ -588,7 +602,7 @@ scan_wp_sum_kernel(const uint8_t* __restrict__ arena, const int64_t* __restrict_
     const uint32_t okbits = wp_decode<false>(R, V, CD, xtab, dd_dst, dd_inf, n, any_raw, lane, nullptr, rec_done);
     const bool vals_ok = __all_sync(FULL, (okbits >> 30) & 1u);
     __syncwarp();
-    cur_off = nxt_off; cur_sz = nxt_sz;
+    if (two) { cur_sz = nb_sz; nb_sz = nxt_sz; stage ^= 1u; R = wb + (stage ? L.rec2 : WP_OFF_REC); } else cur_sz = nxt_sz;
     WPROF(4)                                               // decode (+ the next record's copy issued)
     // zero rows (the last group of an XOR chunk decoded up to 7 rows past the chunk; results of the previous series when O is in V's place)
     if (gz_all) {

@@ -35,9 +35,10 @@ struct WpSmem {                        // byte offsets inside a warp's region, a
   uint32_t rec_cap, vcap /*doubles*/, jcap /*doubles*/, ocap /*doubles*/;
   uint32_t warps;                      // warps per CTA
   uint32_t alias;                      // O lives in V's region: every block of a series is summed (one pass of <= 64 blocks) before the first result is stored
+  uint32_t rec2;                       // second record buffer (0: one): the records of the warp's next two series are in flight
 };
 // wrows = window / step + 1: the most rows a window can span
-FILO_HD inline WpSmem wp_layout(uint32_t max_rec_bytes, uint32_t max_rows, uint32_t max_chunks, uint32_t T, uint32_t wrows, bool alias) {
+FILO_HD inline WpSmem wp_layout(uint32_t max_rec_bytes, uint32_t max_rows, uint32_t max_chunks, uint32_t T, uint32_t wrows, bool alias, bool two_rec = false) {
   WpSmem L;
   if (max_chunks > (uint32_t)WP_MAXC) max_chunks = WP_MAXC;
   L.rec_cap = align_up(max_rec_bytes + 16, 16);
@@ -51,6 +52,8 @@ FILO_HD inline WpSmem wp_layout(uint32_t max_rec_bytes, uint32_t max_rows, uint3
   uint32_t o = WP_OFF_REC;
   L.desc = WP_OFF_DESC; L.jbuf = WP_OFF_J;
   L.rec = o; o += L.rec_cap;
+  L.rec2 = 0;
+  if (two_rec) { L.rec2 = o; o += L.rec_cap; }
   L.vals = o; o += L.vcap * 8;
   if (alias) L.out = L.vals; else { L.out = o; o += L.ocap * 8; }
   L.per_warp = align_up(o, 16);
