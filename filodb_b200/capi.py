@@ -18,7 +18,7 @@ OK, ERR_INVALID_ARG, ERR_CUDA, ERR_CORRUPT_VECTOR, ERR_UNSUPPORTED, ERR_QUERY_LI
 
 EXPORTS = ["filo_ctx_create", "filo_ctx_destroy", "filo_ctx_set_fn_args", "filo_ctx_check", "filo_last_error", "filo_load_series", "filo_table_append", "filo_synth_table", "filo_encode_table", "filo_encode_hist_table", "filo_synth_hist_table",
            "filo_table_set_groups", "filo_table_get_info", "filo_table_read_record", "filo_table_read_arena", "filo_table_free",
-           "filo_num_windows", "filo_query", "filo_query_device", "filo_scan_series", "filo_query_hist", "filo_query_avg_sum_count", "filo_host_register", "filo_host_unregister", "filo_present_partials",
+           "filo_num_windows", "filo_query", "filo_query_device", "filo_scan_series", "filo_query_hist", "filo_query_hist_device", "filo_merge_hist_partials", "filo_query_avg_sum_count", "filo_host_register", "filo_host_unregister", "filo_present_partials",
            "filo_result_max_containers", "filo_encode_result_device", "filo_encode_result"]
 
 
@@ -102,6 +102,10 @@ def _sig(L):
     L.filo_scan_series.argtypes = [vp, i64, vp, vp, i32, i32, i32, i32, i64, i64, i64, i64, vp, C.POINTER(Stats)]
     L.filo_query_hist.restype = i32
     L.filo_query_hist.argtypes = [vp, vp, i32, i64, i64, i64, i64, i32, C.c_double, vp, vp, C.POINTER(Stats)]
+    L.filo_query_hist_device.restype = i32
+    L.filo_query_hist_device.argtypes = [vp, vp, i32, i64, i64, i64, i64, i32, C.c_double, vp, vp, vp, C.POINTER(Stats)]
+    L.filo_merge_hist_partials.restype = i32
+    L.filo_merge_hist_partials.argtypes = [vp, vp, i32, i32, C.c_double, vp, vp, vp, vp]
     L.filo_query_avg_sum_count.restype = i32; L.filo_query_avg_sum_count.argtypes = [vp, vp, vp, i64, i64, i64, i64, vp, C.POINTER(Stats)]
     L.filo_host_register.restype = i32; L.filo_host_register.argtypes = [vp, vp, i64]
     L.filo_host_unregister.restype = i32; L.filo_host_unregister.argtypes = [vp, vp]
@@ -394,6 +398,24 @@ class Context:
         if want_stats:
             self.last_stats = st.as_dict()
         return self.last_stats
+
+    def query_hist_device(self, table, fn, start, step, end, window, d_values=0, d_quantile=0, aggr=AGG_NONE, quantile=None, stream=0, want_stats=True):
+        """filo_query_hist_device: results into device buffers (raw addresses; 0 = not wanted) on `stream`; without want_stats the call
+        does not synchronise and its device-side errors surface at the next call on this ctx or at check()."""
+        st = Stats()
+        self._check(lib().filo_query_hist_device(self.h, table.h, fn, start, step, end, window, aggr, float("nan") if quantile is None else float(quantile),
+                                                 C.c_void_p(d_values) if d_values else None, C.c_void_p(d_quantile) if d_quantile else None,
+                                                 C.c_void_p(stream) if stream else None, C.byref(st) if want_stats else None))
+        if want_stats:
+            self.last_stats = st.as_dict()
+        return self.last_stats
+
+    def merge_hist_partials(self, table, n_parts, n_windows, d_parts, d_out_values=0, d_out_quantile=0, quantile=None, stream=0):
+        """filo_merge_hist_partials: rank-order fold of n_parts histogram SUM partials [n_parts, G, T, nb] (device address) into
+        values [G, T, nb] and / or histogram_quantile [G, T]; `table` supplies G, the buckets and their tops."""
+        self._check(lib().filo_merge_hist_partials(self.h, table.h, n_parts, n_windows, float("nan") if quantile is None else float(quantile),
+                                                   C.c_void_p(d_parts) if d_parts else None, C.c_void_p(d_out_values) if d_out_values else None,
+                                                   C.c_void_p(d_out_quantile) if d_out_quantile else None, C.c_void_p(stream) if stream else None))
 
     def present_partials(self, aggr, n, d_values, d_counts, d_out, stream=0):
         self._check(lib().filo_present_partials(self.h, aggr, n, C.c_void_p(d_values), C.c_void_p(d_counts), C.c_void_p(d_out),

@@ -806,11 +806,30 @@ static int32_t poll_async_errors(filo_ctx* ctx, bool wait) {
   }
   return rc;
 }
+// non-synchronising call: its error word is copied into the next slot of the ring on its stream, so that it still reaches the caller
+// (next call on this ctx, or filo_ctx_check)
+static int32_t push_async_error(filo_ctx* ctx, const int* d_err, cudaStream_t s) {
+  std::lock_guard<std::mutex> g(ctx->errslot_mu);
+  filo_ctx::ErrSlot& sl = ctx->errslots[ctx->errslot_next];
+  ctx->errslot_next = (ctx->errslot_next + 1) % 16;
+  if (!sl.h) { CUDA_TRY(ctx, cudaMallocHost((void**)&sl.h, 16)); CUDA_TRY(ctx, cudaEventCreateWithFlags(&sl.ev, cudaEventDisableTiming)); }
+  if (sl.pending) {           // the ring wrapped: the oldest query must have finished by now
+    CUDA_TRY(ctx, cudaEventSynchronize(sl.ev)); sl.pending = false;
+    if (sl.h[0]) return report_device_error(ctx, sl.h, 0);
+  }
+  CUDA_TRY(ctx, cudaMemcpyAsync(sl.h, d_err, 16, cudaMemcpyDeviceToHost, s));
+  CUDA_TRY(ctx, cudaEventRecord(sl.ev, s));
+  sl.pending = true;
+  return FILO_OK;
+}
 extern "C" int32_t filo_ctx_check(filo_ctx* ctx) {
   if (!ctx) return fail(nullptr, FILO_ERR_INVALID_ARG, "ctx is null");
   return poll_async_errors(ctx, true);
 }
 static int32_t report_device_error(filo_ctx* ctx, const int herr[4], int64_t series_base) {
+  if (herr[0] == 5)           // only the histogram kernels set code 5
+    return fail(ctx, FILO_ERR_UNSUPPORTED, "histogram series with more chunks / sections / rows in range than the device path holds, at series " +
+                std::to_string(series_base + ((int64_t)herr[1] | ((int64_t)herr[2] << 31))));
   const char* what = herr[0] == 4 ? "series needs more decode scratch than the table statistics promised" : "CorruptVector on device";
   return fail(ctx, FILO_ERR_CORRUPT_VECTOR, std::string(what) + " (code " + std::to_string(herr[0]) + ") at series " +
               std::to_string(series_base + ((int64_t)herr[1] | ((int64_t)herr[2] << 31))));
@@ -1022,19 +1041,7 @@ static int32_t query_device_impl(filo_ctx* ctx, const filo_table* t, int32_t fn,
     stats->kernel_launches = launches; stats->h2d_bytes = 0; stats->d2h_bytes = 0;
     if (herr[0]) return report_device_error(ctx, herr, 0);
   }
-  if (!stats && !sink) {      // non-synchronising call: the error word still reaches the caller (next call on this ctx, or filo_ctx_check)
-    std::lock_guard<std::mutex> g(ctx->errslot_mu);
-    filo_ctx::ErrSlot& sl = ctx->errslots[ctx->errslot_next];
-    ctx->errslot_next = (ctx->errslot_next + 1) % 16;
-    if (!sl.h) { CUDA_TRY(ctx, cudaMallocHost((void**)&sl.h, 16)); CUDA_TRY(ctx, cudaEventCreateWithFlags(&sl.ev, cudaEventDisableTiming)); }
-    if (sl.pending) {           // the ring wrapped: the oldest query must have finished by now
-      CUDA_TRY(ctx, cudaEventSynchronize(sl.ev)); sl.pending = false;
-      if (sl.h[0]) return report_device_error(ctx, sl.h, 0);
-    }
-    CUDA_TRY(ctx, cudaMemcpyAsync(sl.h, d_err, 16, cudaMemcpyDeviceToHost, s));
-    CUDA_TRY(ctx, cudaEventRecord(sl.ev, s));
-    sl.pending = true;
-  }
+  if (!stats && !sink) { const int32_t rc = push_async_error(ctx, d_err, s); if (rc != FILO_OK) return rc; }
   if (sink) {           // asynchronous caller: the words land in pinned memory when the stream reaches this point
     sink->launches = launches;
     CUDA_TRY(ctx, cudaMemcpyAsync(sink->herr, d_err, 16, cudaMemcpyDeviceToHost, s));
@@ -1452,8 +1459,11 @@ extern "C" int32_t filo_scan_series(filo_ctx* ctx, int64_t n_series, const int32
 // ------------------------------------------------------------------------------------------------------------------
 // filo_query_hist: PeriodicSamplesMapper over a histogram column (+ HistSumRowAggregator, + histogram_quantile)
 // ------------------------------------------------------------------------------------------------------------------
-static int32_t filo_query_hist_impl(filo_ctx* ctx, const filo_table* t, int32_t fn, int64_t start, int64_t step, int64_t end, int64_t window,
-                                   int32_t agg, double quantile, double* out_values, double* out_quantile, filo_stats* stats) {
+// One orchestration for both entry points.  filo_query_hist_device (host_out false): out_values / out_quantile are device buffers, the call
+// synchronises only when stats != NULL.  filo_query_hist (host_out true): they are host buffers; the results go to device temporaries
+// allocated once every argument has been checked, and their copies to the host are enqueued before the one synchronisation.
+static int32_t hist_query_impl(filo_ctx* ctx, const filo_table* t, int32_t fn, int64_t start, int64_t step, int64_t end, int64_t window,
+                               int32_t agg, double quantile, double* out_values, double* out_quantile, void* cuda_stream, filo_stats* stats, bool host_out) {
   if (!ctx || !t || (!out_values && !out_quantile)) return fail(ctx, FILO_ERR_INVALID_ARG, "filo_query_hist: null argument");
   if (!t->hist) return fail(ctx, FILO_ERR_INVALID_ARG, "filo_query_hist: not a histogram table");
   if (agg != FILO_AGG_NONE && agg != FILO_AGG_SUM) return fail(ctx, FILO_ERR_UNSUPPORTED, "histogram aggregates: sum only");
@@ -1466,7 +1476,8 @@ static int32_t filo_query_hist_impl(filo_ctx* ctx, const filo_table* t, int32_t 
   const bool last = fn == FILO_FN_LAST;
   if (window <= 0) { if (last) window = 5 * 60 * 1000 + 1; else return fail(ctx, FILO_ERR_INVALID_ARG, "Need positive window lengths to apply range function"); }
   CUDA_TRY(ctx, cudaSetDevice(ctx->device));
-  cudaStream_t s = ctx->stream;
+  { const int32_t prc = poll_async_errors(ctx, false); if (prc != FILO_OK) return prc; }      // an earlier stats == NULL query failed on the device
+  cudaStream_t s = cuda_stream ? (cudaStream_t)cuda_stream : ctx->stream;
   const int64_t adjustedStep = step > 0 ? step : step + 1;
   QueryParams q{};
   q.start = start; q.step = adjustedStep; q.end = end; q.window = window; q.T = filo_num_windows(start, adjustedStep, end);
@@ -1490,17 +1501,20 @@ static int32_t filo_query_hist_impl(filo_ctx* ctx, const filo_table* t, int32_t 
   int* d_err = nullptr; unsigned long long* d_counters = nullptr;
   CUDA_TRY(ctx, tmp.alloc((void**)&d_err, 16)); CUDA_TRY(ctx, tmp.alloc((void**)&d_counters, 16));
   CUDA_TRY(ctx, cudaMemsetAsync(d_err, 0, 16, s)); CUDA_TRY(ctx, cudaMemsetAsync(d_counters, 0, 16, s));
-  EventPair evp; CUDA_TRY(ctx, cudaEventCreate(&evp.e0)); CUDA_TRY(ctx, cudaEventCreate(&evp.e1));
+  EventPair evp;
+  if (stats) { CUDA_TRY(ctx, cudaEventCreate(&evp.e0)); CUDA_TRY(ctx, cudaEventCreate(&evp.e1)); }
   cudaEvent_t& e0 = evp.e0; cudaEvent_t& e1 = evp.e1;
   const int64_t work = fused ? t->n_items : t->n_series;
   ScanLaunch L{t->d_arena, t->d_rec_off, t->n_series, q, nullptr, 0, 0, d_counters, d_err, 1, s};
   const int ctas_per_sm = (int)std::max<size_t>(1, (size_t)(228 * 1024) / (smem + 2048));
   L.grid = (int)std::max<int64_t>(1, std::min<int64_t>(work, (int64_t)ctx->sm_count * ctas_per_sm));
   const int64_t rows = fused ? t->n_groups : t->n_series;
-  double *d_out = nullptr, *d_q = nullptr, *pval = nullptr; uint8_t* pany = nullptr;
-  if (out_values) CUDA_TRY(ctx, tmp.alloc((void**)&d_out, (size_t)rows * T * nb * 8));
-  if (out_quantile) CUDA_TRY(ctx, tmp.alloc((void**)&d_q, (size_t)rows * T * 8));
-  CUDA_TRY(ctx, cudaEventRecord(e0, s));
+  double *d_out = out_values, *d_q = out_quantile, *pval = nullptr; uint8_t* pany = nullptr;
+  if (host_out) {
+    if (out_values) CUDA_TRY(ctx, tmp.alloc((void**)&d_out, (size_t)rows * T * nb * 8));
+    if (out_quantile) CUDA_TRY(ctx, tmp.alloc((void**)&d_q, (size_t)rows * T * 8));
+  }
+  if (stats) CUDA_TRY(ctx, cudaEventRecord(e0, s));
   if (v2 && !fused) {
     const int cps = (int)std::max<size_t>(1, std::min<size_t>(2, (size_t)(228 * 1024) / (smem2 + 1024)));
     L.grid = (int)std::max<int64_t>(1, std::min<int64_t>(hist2_series_items(t->n_series), (int64_t)ctx->sm_count * cps));
@@ -1522,29 +1536,51 @@ static int32_t filo_query_hist_impl(filo_ctx* ctx, const filo_table* t, int32_t 
   } else {
     CUDA_TRY(ctx, launch_hist_scan(L, nb, t->max_rows, t->max_rec_bytes, nullptr, nullptr, 0, 0, d_out, nullptr, nullptr, t->d_hist_tops, quantile, t->hist_exp ? 1 : 0, d_q));
   }
+  if (!stats) return push_async_error(ctx, d_err, s);
   CUDA_TRY(ctx, cudaEventRecord(e1, s));
   int herr[4]; unsigned long long hc[2];
   CUDA_TRY(ctx, cudaMemcpyAsync(herr, d_err, 16, cudaMemcpyDeviceToHost, s));
   CUDA_TRY(ctx, cudaMemcpyAsync(hc, d_counters, 16, cudaMemcpyDeviceToHost, s));
-  if (out_values) CUDA_TRY(ctx, cudaMemcpyAsync(out_values, d_out, (size_t)rows * T * nb * 8, cudaMemcpyDeviceToHost, s));
-  if (out_quantile) CUDA_TRY(ctx, cudaMemcpyAsync(out_quantile, d_q, (size_t)rows * T * 8, cudaMemcpyDeviceToHost, s));
+  const size_t d2h = host_out ? (out_values ? (size_t)rows * T * nb * 8 : 0) + (out_quantile ? (size_t)rows * T * 8 : 0) : 0;
+  if (host_out && out_values) CUDA_TRY(ctx, cudaMemcpyAsync(out_values, d_out, (size_t)rows * T * nb * 8, cudaMemcpyDeviceToHost, s));
+  if (host_out && out_quantile) CUDA_TRY(ctx, cudaMemcpyAsync(out_quantile, d_q, (size_t)rows * T * 8, cudaMemcpyDeviceToHost, s));
   CUDA_TRY(ctx, cudaStreamSynchronize(s));
   float ms = 0; cudaEventElapsedTime(&ms, e0, e1);
-  if (stats) {
-    stats->kernel_ns = (int64_t)((double)ms * 1e6); stats->samples_scanned = (int64_t)hc[0]; stats->bytes_scanned = (int64_t)hc[1];
-    stats->kernel_launches = fused ? 2 : 1; stats->h2d_bytes = 0;
-    stats->d2h_bytes = (int64_t)((out_values ? (size_t)rows * T * nb * 8 : 0) + (out_quantile ? (size_t)rows * T * 8 : 0));
-  }
-  if (herr[0] == 5) return fail(ctx, FILO_ERR_UNSUPPORTED, "histogram series with more chunks / sections / rows in range than the device path holds, at series " +
-                                std::to_string((int64_t)herr[1] | ((int64_t)herr[2] << 31)));
+  stats->kernel_ns = (int64_t)((double)ms * 1e6); stats->samples_scanned = (int64_t)hc[0]; stats->bytes_scanned = (int64_t)hc[1];
+  stats->kernel_launches = fused ? 2 : 1; stats->h2d_bytes = 0; stats->d2h_bytes = (int64_t)d2h;
   if (herr[0]) return report_device_error(ctx, herr, 0);
   return FILO_OK;
 }
-extern "C" int32_t filo_query_hist(filo_ctx* ctx, const filo_table* t, int32_t fn, int64_t start, int64_t step, int64_t end, int64_t window,
-                                   int32_t agg, double quantile, double* out_values, double* out_quantile, filo_stats* stats) {
-  try { return filo_query_hist_impl(ctx, t, fn, start, step, end, window, agg, quantile, out_values, out_quantile, stats); }
+extern "C" int32_t filo_query_hist_device(filo_ctx* ctx, const filo_table* t, int32_t fn, int64_t start, int64_t step, int64_t end, int64_t window,
+                                          int32_t agg, double quantile, void* d_out_values, void* d_out_quantile, void* cuda_stream, filo_stats* stats) {
+  try { return hist_query_impl(ctx, t, fn, start, step, end, window, agg, quantile, (double*)d_out_values, (double*)d_out_quantile, cuda_stream, stats, false); }
   catch (const std::bad_alloc&) { return fail(ctx, FILO_ERR_OOM, "filo_query_hist: host allocation failed"); }
   catch (const std::exception& e) { return fail(ctx, FILO_ERR_INVALID_ARG, std::string("filo_query_hist: ") + e.what()); }
+}
+extern "C" int32_t filo_query_hist(filo_ctx* ctx, const filo_table* t, int32_t fn, int64_t start, int64_t step, int64_t end, int64_t window,
+                                   int32_t agg, double quantile, double* out_values, double* out_quantile, filo_stats* stats) {
+  filo_stats st{};         // the host form always synchronises
+  try { const int32_t rc = hist_query_impl(ctx, t, fn, start, step, end, window, agg, quantile, out_values, out_quantile, nullptr, &st, true);
+        if (stats) *stats = st;
+        return rc; }
+  catch (const std::bad_alloc&) { return fail(ctx, FILO_ERR_OOM, "filo_query_hist: host allocation failed"); }
+  catch (const std::exception& e) { return fail(ctx, FILO_ERR_INVALID_ARG, std::string("filo_query_hist: ") + e.what()); }
+}
+
+extern "C" int32_t filo_merge_hist_partials(filo_ctx* ctx, const filo_table* t, int32_t n_parts, int32_t n_windows, double quantile,
+                                            const void* d_parts, void* d_out_values, void* d_out_quantile, void* cuda_stream) {
+  if (!ctx || !t || !d_parts) return fail(ctx, FILO_ERR_INVALID_ARG, "filo_merge_hist_partials: null argument");
+  if (!t->hist) return fail(ctx, FILO_ERR_INVALID_ARG, "filo_merge_hist_partials: not a histogram table");
+  if (n_parts < 1 || n_windows < 1) return fail(ctx, FILO_ERR_INVALID_ARG, "filo_merge_hist_partials: n_parts and n_windows must be >= 1");
+  double* d_q = quantile == quantile ? (double*)d_out_quantile : nullptr;              // quantile NaN: the values alone
+  if (!d_out_values && !d_q) return fail(ctx, FILO_ERR_INVALID_ARG, "filo_merge_hist_partials: no output (values NULL, and quantile NaN or its output NULL)");
+  if (t->hist_nb > 64) return fail(ctx, FILO_ERR_UNSUPPORTED, "filo_merge_hist_partials: more than 64 buckets");
+  CUDA_TRY(ctx, cudaSetDevice(ctx->device));
+  { const int32_t prc = poll_async_errors(ctx, false); if (prc != FILO_OK) return prc; }      // e.g. the query that produced a part failed
+  cudaStream_t s = cuda_stream ? (cudaStream_t)cuda_stream : ctx->stream;
+  CUDA_TRY(ctx, launch_hist_merge_parts((const double*)d_parts, n_parts, (int64_t)t->n_groups * n_windows, t->hist_nb, t->hist_exp ? 1 : 0, t->d_hist_tops,
+                                        quantile, (double*)d_out_values, d_q, s));
+  return FILO_OK;
 }
 
 extern "C" int32_t filo_present_partials(filo_ctx* ctx, int32_t agg, int64_t n, void* d_values, void* d_counts, void* d_out, void* cuda_stream) {

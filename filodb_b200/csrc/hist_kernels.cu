@@ -469,8 +469,7 @@ __global__ void hist_merge_kernel(const double* __restrict__ pval, const uint8_t
     if (!pany[(size_t)it * T + k]) continue;
     const double* pv = pval + ((size_t)it * T + k) * nb;
     if (!any) { for (int b = 0; b < nb; ++b) v[b] = pv[b]; any = true; continue; }
-    double mx = 0.0;
-    for (int b = 0; b < nb; ++b) { double nv = v[b] + pv[b]; if (nv < mx || nv != nv) nv = mx; else if (nv > mx) mx = nv; v[b] = nv; }
+    hist_add_monotonic(v, pv, 1, nb);
   }
   const double qv = (any && qtl == qtl) ? hist_quantile(v, nb, tops, qtl, exp_buckets != 0) : NaNv;
   if (out_values) for (int b = 0; b < nb; ++b) out_values[(size_t)i * nb + b] = any ? v[b] : NaNv;

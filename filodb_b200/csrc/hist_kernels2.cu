@@ -152,12 +152,34 @@ __global__ void hist_merge2_kernel(const double* __restrict__ pval, const uint8_
     if (!pany[(size_t)it * T + k]) continue;
     const double* pv = pval + (size_t)it * T * nb + k;
     if (!any) { for (int b = 0; b < nb; ++b) v[b] = pv[(size_t)b * T]; any = true; continue; }
-    double mx = 0.0;
-    for (int b = 0; b < nb; ++b) { double nv = v[b] + pv[(size_t)b * T]; if (nv < mx || nv != nv) nv = mx; else if (nv > mx) mx = nv; v[b] = nv; }
+    hist_add_monotonic(v, pv, (size_t)T, nb);
   }
   const double qv = (any && qtl == qtl) ? hist_quantile(v, nb, tops, qtl, exp_buckets != 0) : NaNv;
   if (out_values) for (int b = 0; b < nb; ++b) out_values[(size_t)i * nb + b] = any ? v[b] : NaNv;
   if (out_q) out_q[i] = qv;
+}
+
+// The cross-GPU reduce of histogram sums (filo_merge_hist_partials): parts holds n_parts SUM outputs of filo_query_hist_device back to
+// back, [n_parts][n_cells][nb] with n_cells = G * T, in rank order.  A part's cell is empty when its bucket 0 is NaN: a SUM output is NaN
+// in every bucket where its group had no histogram, and never NaN in bucket 0 otherwise (integer-count inputs give finite window
+// histograms, and makeMonotonic replaces a NaN by the running maximum, which starts at 0).  ReduceAggregateExec with
+// HistSumRowAggregator.reduceAggregate folds the parts in rank order: the first non-empty one is copied, every further one goes through
+// hist_add_monotonic.  Then Histogram.quantile when out_q is given.  Thread per (group, window).
+__global__ void hist_merge_parts_kernel(const double* __restrict__ parts, int n_parts, int64_t n_cells, int nb, int exp_buckets,
+                                        const double* __restrict__ tops, double qtl,
+                                        double* __restrict__ out_values /* [G][T][nb] or null */, double* __restrict__ out_q /* [G][T] or null */) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n_cells) return;
+  const double NaNv = __longlong_as_double(0x7ff8000000000000LL);
+  double v[64]; bool any = false;
+  for (int p = 0; p < n_parts; ++p) {
+    const double* pv = parts + ((size_t)p * (size_t)n_cells + (size_t)i) * nb;
+    if (pv[0] != pv[0]) continue;                                  // Histogram.empty on this rank
+    if (!any) { for (int b = 0; b < nb; ++b) v[b] = pv[b]; any = true; continue; }
+    hist_add_monotonic(v, pv, 1, nb);
+  }
+  if (out_values) for (int b = 0; b < nb; ++b) out_values[(size_t)i * nb + b] = any ? v[b] : NaNv;
+  if (out_q) out_q[i] = any ? hist_quantile(v, nb, tops, qtl, exp_buckets != 0) : NaNv;
 }
 
 #ifndef FILO_CUSIM      // launchers need nvcc
@@ -198,6 +220,12 @@ cudaError_t launch_hist_merge2(const double* pval, const uint8_t* pany, const in
   const int64_t n = (int64_t)n_groups * T;
   if (n <= 0) return cudaSuccess;
   hist_merge2_kernel<<<(unsigned)((n + 127) / 128), 128, 0, s>>>(pval, pany, gis, n_groups, T, nb, exp_buckets, tops, q, out_values, out_q);
+  return cudaGetLastError();
+}
+cudaError_t launch_hist_merge_parts(const double* parts, int n_parts, int64_t n_cells, int nb, int exp_buckets, const double* tops, double q,
+                                    double* out_values, double* out_q, cudaStream_t s) {
+  if (n_cells <= 0) return cudaSuccess;
+  hist_merge_parts_kernel<<<(unsigned)((n_cells + 127) / 128), 128, 0, s>>>(parts, n_parts, n_cells, nb, exp_buckets, tops, q, out_values, out_q);
   return cudaGetLastError();
 }
 

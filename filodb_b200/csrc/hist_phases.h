@@ -470,6 +470,14 @@ FILO_HD inline bool h2_window_last(int k, const H2Ctx& X, double* pv, bool first
   return true;
 }
 
+// MutableHistogram.add of a further histogram p[b * ps] into the running sum v (Histogram.scala:428-449): addNoCorrection, a bucket-wise
+// sum, then makeMonotonic: a bucket below the running maximum, or NaN, becomes that maximum.  The step of every merge kernel
+// (hist_merge_kernel, hist_merge2_kernel, hist_merge_parts_kernel); the first histogram of a fold is copied, not added.
+FILO_HDI void hist_add_monotonic(double* v, const double* p, size_t ps, int nb) {
+  double mx = 0.0;
+  for (int b = 0; b < nb; ++b) { double nv = v[b] + p[(size_t)b * ps]; if (nv < mx || nv != nv) nv = mx; else if (nv > mx) mx = nv; v[b] = nv; }
+}
+
 // Histogram.quantile (vectors/Histogram.scala:65-108; min = 0, max = +Inf, evenDistribution = false) over cumulative bucket sums v[b * vs]
 // with bucket tops tops[nb]; exp_buckets: Base2ExpHistogramBuckets interpolate in log2 space except in the zero bucket (:97-104, log2 :111).
 // No makeMonotonic: firstBucketGTE walks up from bucket 0 as the reference does, also over a non-monotonic per-series histogram.

@@ -74,6 +74,9 @@ cudaError_t launch_hist_scan2_series(const ScanLaunch& L, int nb, int max_rows, 
                                      const double* tops, double qtl, int exp_buckets);
 cudaError_t launch_hist_merge2(const double* pval, const uint8_t* pany, const int64_t* gis, int n_groups, int T, int nb, int exp_buckets, const double* tops, double q,
                                double* out_values, double* out_q, cudaStream_t s);
+// rank-order fold of n_parts histogram SUM outputs [n_parts][n_cells][nb] (empty cell: NaN bucket 0), histogram_quantile when out_q is given
+cudaError_t launch_hist_merge_parts(const double* parts, int n_parts, int64_t n_cells, int nb, int exp_buckets, const double* tops, double q,
+                                    double* out_values, double* out_q, cudaStream_t s);
 cudaError_t launch_iota(int32_t* a, int64_t n, cudaStream_t s);
 cudaError_t launch_group_bounds(const int32_t* sorted_keys, int64_t n, int n_groups, int64_t* group_start, cudaStream_t s);
 cudaError_t launch_group_item_count(const int64_t* group_start, int n_groups, int seg, int64_t* cnt, cudaStream_t s);

@@ -3,7 +3,8 @@
 One process per GPU.  Series are independent until the across-series aggregate (SURVEY.md §8e), so the data path has no
 collective for per-series queries; aggregates merge `[G x T]` partials (FILO_Q_PARTIAL form, include/filo_b200.h) with
 one all-reduce, the role `LocalPartitionReduceAggregateExec` + `RowAggregator.reduceAggregate` play in the reference
-(query/exec/AggrOverRangeVectors.scala:119-182; aggregator/*RowAggregator.scala).
+(query/exec/AggrOverRangeVectors.scala:119-182; aggregator/*RowAggregator.scala).  Histogram sums are gathered instead
+(gather_hist_partials) and folded in rank order on the device by filo_merge_hist_partials.
 
 Works on CUDA tensors over NCCL (product) and on CPU tensors over gloo (tests/test_multi_gpu_gloo.py).
 """
@@ -42,6 +43,18 @@ def merge_partials(values, counts, aggr_op: int, dist) -> None:
     else:
         raise ValueError("aggregate %d has no all-reduce merge (topk merges gathered candidates)" % aggr_op)
     dist.all_reduce(counts, op=dist.ReduceOp.SUM)
+
+
+def gather_hist_partials(values, dist):
+    """Every rank's histogram SUM partial (filo_query_hist_device with aggr SUM, [G, T, nb] f64, NaN buckets = empty) -> [W, G, T, nb]
+    in rank order, for filo_merge_hist_partials.  all_gather into views of one preallocated tensor, so the same code runs on gloo
+    (CPU tensors) and NCCL (CUDA tensors)."""
+    import torch
+    # A gather, not an all-reduce: HistSumRowAggregator.reduceAggregate copies the first non-empty histogram and makes every later sum
+    # monotonic (MutableHistogram.add, Histogram.scala:428-451), so the merge is an ordered fold that a reduction op cannot express.
+    out = torch.empty((dist.get_world_size(),) + tuple(values.shape), dtype=values.dtype, device=values.device)
+    dist.all_gather(list(out.unbind(0)), values.contiguous())
+    return out
 
 
 def max_over_ranks(x: float, dist, device) -> float:

@@ -274,6 +274,30 @@ int32_t filo_query_avg_sum_count(filo_ctx* ctx, const filo_table* t_sum, const f
 int32_t filo_query_hist(filo_ctx* ctx, const filo_table* t, int32_t range_fn,
                         int64_t start_ms, int64_t step_ms, int64_t end_ms, int64_t window_ms,
                         int32_t aggr_op, double quantile, double* out_values, double* out_quantile, filo_stats* stats);
+/* Same, results left in DEVICE buffers (d_out_values / d_out_quantile are device pointers, either may be NULL as above), enqueued on
+ * cuda_stream (a cudaStream_t, may be NULL = ctx stream) with its temporaries stream-ordered on it; does not synchronize unless
+ * stats != NULL.  Device-side errors of a call with stats == NULL (CorruptVector, or a series with more chunks / sections / rows in
+ * range than the device path holds) are returned by the next call on the ctx that finds them complete, or by filo_ctx_check, with the
+ * status and message the synchronous call returns.  filo_query_hist runs the same code into device temporaries (allocated only once the
+ * arguments have been checked) and copies them to the host before its one synchronisation.
+ * aggr SUM without a quantile gives the per-GPU partial of the cross-GPU histogram sum: [n_groups * T * buckets], NaN in every bucket
+ * of an empty cell, never NaN in bucket 0 of a non-empty one (the device path reads integer-count histograms only, and makeMonotonic
+ * replaces NaN).  Gather the partials of all ranks (not an all-reduce: the fold below is not a sum) and call filo_merge_hist_partials. */
+int32_t filo_query_hist_device(filo_ctx* ctx, const filo_table* t, int32_t range_fn,
+                               int64_t start_ms, int64_t step_ms, int64_t end_ms, int64_t window_ms,
+                               int32_t aggr_op, double quantile, void* d_out_values, void* d_out_quantile, void* cuda_stream, filo_stats* stats);
+/* ReduceAggregateExec of histogram sums across GPUs: d_parts holds n_parts aggr SUM outputs of filo_query_hist_device back to back,
+ * [n_parts][n_groups][n_windows][buckets] doubles in DEVICE memory, in rank order.  For every (group, window) the parts are folded in
+ * that order with HistSumRowAggregator.reduceAggregate: empty cells (bucket 0 NaN) are skipped, the first non-empty one is copied and
+ * every further one goes through MutableHistogram.add (bucket-wise sum + makeMonotonic, Histogram.scala:428-449); then
+ * histogram_quantile.  d_out_values [n_groups * n_windows * buckets] (NaN buckets for a cell empty on every rank) and
+ * d_out_quantile [n_groups * n_windows] as filo_query_hist's SUM outputs; either may be NULL, and a NaN quantile writes the values alone.
+ * Caller's contract: t is any rank's table over the same bucket scheme and the same group numbering (n_groups, the bucket count, the
+ * bucket tops and the exponential flag come from it), and every part was computed with the same start / step / end.
+ * Enqueued on cuda_stream (NULL = ctx stream), no synchronisation.  FILO_ERR_INVALID_ARG for n_parts < 1, n_windows < 1, a table that
+ * is not a histogram table, or no output; FILO_ERR_UNSUPPORTED for more than 64 buckets. */
+int32_t filo_merge_hist_partials(filo_ctx* ctx, const filo_table* t, int32_t n_parts, int32_t n_windows, double quantile,
+                                 const void* d_parts, void* d_out_values, void* d_out_quantile, void* cuda_stream);
 
 /* Registers a region of host memory that holds chunk vectors (FiloDB's off-heap block memory, BlockManager pages) for direct
  * device access: pinned + mapped once, like the reference maps its blocks once at start-up.  filo_scan_series then lets the
