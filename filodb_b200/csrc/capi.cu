@@ -933,7 +933,8 @@ static int32_t query_device_impl(filo_ctx* ctx, const filo_table* t, int32_t fn,
   }
   // v4 SUM kernel (scan_wp.cuh): per-series rows, in front of the tile kernel; what it declines goes to the v2 kernel
   WpSmem WL{};
-  bool use_wp = false;
+  WpBatchSmem WB{};
+  bool use_wp = false, use_wp_batch = false;
   if (use_tile && force != "v3" && wrows <= 4096 && t->max_chunks > 0) {
     // O in V's place (more warps per SM) when every series is summed in one pass of <= 64 blocks
     const bool alias = wp_max_items((uint32_t)t->max_chunks, (uint32_t)q.T, (uint32_t)wrows) <= 64;
@@ -941,7 +942,12 @@ static int32_t query_device_impl(filo_ctx* ctx, const filo_table* t, int32_t fn,
     WL.warps = (uint32_t)std::min<size_t>(smem_cap / WL.per_warp, alias ? WP_MAX_WARPS_ALIAS : WP_MAX_WARPS);
     // two record buffers per warp (the records of the next two series in flight) when 16 warps of them fit
     const WpSmem WL2 = wp_layout(t->max_rec_bytes, (uint32_t)t->max_rows, (uint32_t)t->max_chunks, (uint32_t)q.T, (uint32_t)wrows, alias, true);
-    if (smem_cap / WL2.per_warp >= (size_t)WP_MAX_WARPS) { WL = WL2; WL.warps = WP_MAX_WARPS; }
+    if (smem_cap / WL2.per_warp >= (size_t)WP_MAX_WARPS) {
+      WL = WL2; WL.warps = WP_MAX_WARPS;
+      // that layout's record bytes as one CTA-wide stream: batches of consecutive records, a producer warp parses their headers
+      WB = wp_batch_layout(t->max_rec_bytes, (uint32_t)t->max_rows, (uint32_t)t->max_chunks, (uint32_t)q.T, (uint32_t)wrows, alias);
+      use_wp_batch = WB.total <= smem_cap;
+    }
     use_wp = WL.warps >= 4;
   }
   // v4 counter-class kernel (scan_wp_ctr.cuh): per-series rows, or fused partial rows of up to TILE_AGG_ACC * TILE_THREADS windows;
@@ -964,7 +970,10 @@ static int32_t query_device_impl(filo_ctx* ctx, const filo_table* t, int32_t fn,
       CUDA_TRY(ctx, cudaMemsetAsync(d_cnt, 0, 16, s));
       ScanLaunch LT = L;
       static const bool dbg = std::getenv("FILO_DEBUG_SYNC") != nullptr;
-      if (use_wp) {
+      if (use_wp_batch) {
+        LT.grid = (int)std::max<int64_t>(1, std::min<int64_t>((t->n_series + WB.B - 1) / WB.B, (int64_t)ctx->sm_count));
+        CUDA_TRY(ctx, launch_scan_wp_batch(LT, outp, WB, d_list, d_cnt));
+      } else if (use_wp) {
         LT.grid = (int)std::max<int64_t>(1, std::min<int64_t>((t->n_series + WL.warps - 1) / WL.warps, (int64_t)ctx->sm_count));
         CUDA_TRY(ctx, launch_scan_wp(LT, outp, WL, d_list, d_cnt));
       } else if (use_wp_ctr) {

@@ -53,6 +53,8 @@ cudaError_t launch_topk(const double* per_series, const int32_t* order, const in
                         double* out_val, int64_t* out_id, cudaStream_t s);
 struct WpSmem;
 cudaError_t launch_scan_wp(const ScanLaunch& L, double* out, const WpSmem& W, int64_t* fallback_list, unsigned long long* fallback_count);
+struct WpBatchSmem;
+cudaError_t launch_scan_wp_batch(const ScanLaunch& L, double* out, const WpBatchSmem& W, int64_t* fallback_list, unsigned long long* fallback_count);
 struct WpCtrSmem;
 cudaError_t launch_scan_wp_ctr(const ScanLaunch& L, double* out, const WpCtrSmem& W, int64_t* fallback_list, unsigned long long* fallback_count);
 cudaError_t launch_scan_wp_ctr_agg(const ScanLaunch& L, const WpCtrSmem& W, const int32_t* order, const int64_t* item_begin, int64_t n_items, int agg_op,

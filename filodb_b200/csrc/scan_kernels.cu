@@ -439,9 +439,9 @@ extern "C" int filo_debug_tile_prof(unsigned long long* out16, int reset) {
 }
 #endif
 #ifdef FILO_WP_PROF
-extern "C" int filo_debug_wp_prof(unsigned long long* out16, int reset) {
-  cudaError_t e = cudaMemcpyFromSymbol(out16, g_wp_prof, sizeof(unsigned long long) * 16);
-  if (e == cudaSuccess && reset) { unsigned long long z[16] = {}; e = cudaMemcpyToSymbol(g_wp_prof, z, sizeof z); }
+extern "C" int filo_debug_wp_prof(unsigned long long* out32, int reset) {
+  cudaError_t e = cudaMemcpyFromSymbol(out32, g_wp_prof, sizeof(unsigned long long) * 32);
+  if (e == cudaSuccess && reset) { unsigned long long z[32] = {}; e = cudaMemcpyToSymbol(g_wp_prof, z, sizeof z); }
   return (int)e;
 }
 #endif
@@ -542,6 +542,23 @@ cudaError_t launch_scan_wp(const ScanLaunch& L, double* out, const WpSmem& W, in
     case FN_AVG: return launch_wp_fn<FN_AVG>(L, out, W, fallback_list, fallback_count);
     case FN_COUNT: return launch_wp_fn<FN_COUNT>(L, out, W, fallback_list, fallback_count);
     default: return launch_wp_fn<FN_SUM>(L, out, W, fallback_list, fallback_count);      // FN_SUM, FN_INCREASE on a delta schema
+  }
+}
+// the same with a CTA-wide record stream (scan_wp_batch_kernel): 15 consumer warps + 1 producer warp per SM
+template <int FN>
+static cudaError_t launch_wp_batch_fn(const ScanLaunch& L, double* out, const WpBatchSmem& W, int64_t* fallback_list, unsigned long long* fallback_count) {
+  cudaError_t e = cudaFuncSetAttribute(scan_wp_batch_kernel<FN, WP_BATCH_WARPS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)W.total);
+  if (e != cudaSuccess) return e;
+  scan_wp_batch_kernel<FN, WP_BATCH_WARPS><<<L.grid, WP_BATCH_WARPS * 32, W.total, L.stream>>>(L.arena, L.rec_off, L.n_series, L.q, out, W, fallback_list,
+      fallback_count, L.d_counters, L.d_err);
+  return cudaGetLastError();
+}
+cudaError_t launch_scan_wp_batch(const ScanLaunch& L, double* out, const WpBatchSmem& W, int64_t* fallback_list, unsigned long long* fallback_count) {
+  switch (L.q.fn) {
+    case FN_RATE: return launch_wp_batch_fn<FN_RATE>(L, out, W, fallback_list, fallback_count);
+    case FN_AVG: return launch_wp_batch_fn<FN_AVG>(L, out, W, fallback_list, fallback_count);
+    case FN_COUNT: return launch_wp_batch_fn<FN_COUNT>(L, out, W, fallback_list, fallback_count);
+    default: return launch_wp_batch_fn<FN_SUM>(L, out, W, fallback_list, fallback_count);      // FN_SUM, FN_INCREASE on a delta schema
   }
 }
 // v4 counter-class kernel (scan_wp_ctr.cuh): per-series rows (order == nullptr, n_items == 0) or one partial row per work item

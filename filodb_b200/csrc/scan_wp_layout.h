@@ -61,6 +61,58 @@ FILO_HD inline WpSmem wp_layout(uint32_t max_rec_bytes, uint32_t max_rows, uint3
   L.alias = alias ? 1u : 0u;
   return L;
 }
+
+// SUM-class kernel with a CTA-wide record stream (scan_wp_batch_kernel): 15 consumer warps and 1 producer warp (16 warps x 128 registers).
+// The producer fetches batches of WP_BATCH_SERIES consecutive records into WP_BATCH_BUFS batch buffers: 30 records per CTA, the record
+// bytes of two buffers per warp at 15 warps.  On C2, 15 x 2 ran 4 % faster than 5 x 6 (DESIGN §4.1).
+constexpr int WP_BATCH_WARPS = 16;
+constexpr int WP_BATCH_SERIES = 15;
+constexpr int WP_BATCH_BUFS = 2;
+struct WpEntryChunk {                  // what the producer's header parse found of one chunk in range (zero for chunks c >= n)
+  uint64_t first;                      // XOR: bits of the first value; raw f64: the first value
+  int64_t init, end_time;              // with nrows and wire: the memo key of the window plan
+  uint32_t grp_off, val_off;           // byte offsets in the record: first group (XOR), value vector
+  int32_t nrows, grp_base, ng;         // rows, group slots [grp_base, grp_base + ng)
+  uint32_t wire;                       // value vector wire | drop flag << 16
+};
+static_assert(sizeof(WpEntryChunk) == 48, "WpEntryChunk");
+struct WpEntry {                       // one series of a batch (shared memory, written by the producer, read by one consumer warp)
+  uint32_t rofs;                       // the record's byte offset in the batch buffer
+  int32_t n;                           // chunks in range
+  int32_t flags;                       // bit 0: regular as far as the header goes (wp_parse), bit 1: a chunk has raw f64 values
+  int32_t ngroups, cnt_rows, cnt_bytes;   // NibblePack groups; the series' scan counters
+  int32_t pad[2];
+  WpEntryChunk c[WP_MAXC];
+};
+static_assert(sizeof(WpEntry) == 224, "WpEntry");
+struct WpBatchSmem {                   // byte offsets inside the CTA's shared memory, all multiples of 16
+  WpSmem W;                            // a consumer warp's region: wp_layout without record buffers (V at WP_OFF_REC)
+  uint32_t B, nbuf, consumers;         // series per batch, batch buffers, consumer warps (the producer is warp `consumers`)
+  uint32_t buf, buf_stride, buf_cap;   // batch buffer b at buf + b * buf_stride; a batch is staged when its records take <= buf_cap bytes
+  uint32_t ent;                        // WpEntry[nbuf][B]
+  uint32_t bars;                       // mbarriers full[nbuf], parsed[nbuf], empty[nbuf]
+  uint32_t total;                      // bytes per CTA
+};
+FILO_HD inline WpBatchSmem wp_batch_layout(uint32_t max_rec_bytes, uint32_t max_rows, uint32_t max_chunks, uint32_t T, uint32_t wrows, bool alias,
+                                           uint32_t B = WP_BATCH_SERIES, uint32_t nbuf = WP_BATCH_BUFS, uint32_t consumers = WP_BATCH_WARPS - 1) {
+  WpBatchSmem S;
+  WpSmem L = wp_layout(max_rec_bytes, max_rows, max_chunks, T, wrows, alias);
+  const uint32_t shift = L.vals - WP_OFF_REC;                                 // the record buffer leaves the warp's region
+  L.vals -= shift; L.out -= shift; L.per_warp -= shift; L.rec = 0;
+  S.consumers = consumers;
+  L.warps = S.consumers;
+  S.W = L; S.B = B; S.nbuf = nbuf;
+  uint32_t o = L.per_warp * S.consumers;
+  S.buf = o;
+  S.buf_cap = B * align_up(max_rec_bytes, 16);                                // records are 16-byte aligned and adjacent in the arena
+  S.buf_stride = S.buf_cap + 16;                                              // (the group decode reads up to 8 bytes past a record)
+  o += nbuf * S.buf_stride;
+  S.ent = o; o += nbuf * B * (uint32_t)sizeof(WpEntry);
+  S.bars = o; o += 3 * nbuf * 8;
+  S.total = align_up(o, 16);
+  return S;
+}
+
 // an upper bound of the blocks of a series: sum over chunks of ceil(touched windows / 8), with at most wrows - 1 windows shared per junction
 FILO_HD inline uint32_t wp_max_items(uint32_t max_chunks, uint32_t T, uint32_t wrows) {
   if (max_chunks > (uint32_t)WP_MAXC) max_chunks = WP_MAXC;
