@@ -21,9 +21,17 @@
 
 namespace filo {
 
+// bulk store shared -> global (one bulk group): both addresses 16-byte aligned, size a nonzero multiple of 16 (checked on the emulator)
 #ifdef FILO_CUSIM
-inline void tma_store_1d(void* gdst, const void* ssrc, uint32_t bytes) { cusim::tma_store(gdst, ssrc, bytes); }
+inline void tma_store_1d(void* gdst, const void* ssrc, uint32_t bytes) {
+  if ((reinterpret_cast<uintptr_t>(gdst) & 15) || (reinterpret_cast<uintptr_t>(ssrc) & 15) || bytes == 0 || (bytes & 15)) {
+    std::fprintf(stderr, "cusim: bulk store of %u bytes from %p to %p: needs 16-byte alignment and a nonzero multiple of 16 bytes\n", bytes, ssrc, gdst);
+    std::abort();
+  }
+  cusim::tma_store(gdst, ssrc, bytes);
+}
 inline void tma_store_wait_read() { cusim::tma_store_wait_read(); }
+inline void tma_store_wait_all() { cusim::tma_store_wait_read(); }
 inline void fence_async_smem() {}
 #else
 __device__ __forceinline__ void tma_store_1d(void* gdst, const void* ssrc, uint32_t bytes) {
@@ -31,6 +39,7 @@ __device__ __forceinline__ void tma_store_1d(void* gdst, const void* ssrc, uint3
   asm volatile("cp.async.bulk.commit_group;" ::: "memory");
 }
 __device__ __forceinline__ void tma_store_wait_read() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
+__device__ __forceinline__ void tma_store_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
 __device__ __forceinline__ void fence_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 #endif
 

@@ -21,7 +21,8 @@
 //            partial sum from each chunk's block list (the earlier chunk's in O, the later one's in J);
 //   finish   lane l = windows l + 32 m: one pass loads O (and J), finishes by the window's class (junction sums in chunk order, raw
 //            sums, windows without rows) and stores straight to the output: lane-consecutive streaming stores, 256 contiguous bytes
-//            per store instruction.  Nothing is written back to O.
+//            per store instruction.  Nothing is written back to O.  scan_wp_batch_kernel instead writes the finished row over O and
+//            stores it with one bulk copy (wp_finish_store<FN, true>).
 // Anything outside this fast path (irregular timestamps, DDV-long values, > 4 chunks, NaN / Inf / denormal / zero values, windows
 // shorter than 9 rows, windows over three chunks ...) is appended to the fallback list and answered by the v2 kernel into the same
 // output buffer, exactly as the tile kernel does.
@@ -41,8 +42,8 @@ __device__ __forceinline__ uint32_t wp_lds32(uint32_t off) { uint32_t v; asm vol
 #endif
 
 // Per-phase cycle counters of the SUM-class kernels for profiling builds (-DFILO_WP_PROF; scratch/wp_prof.py): every lane reads the
-// SM clock at the phase boundaries of a series, lane 0 adds its sums to g_wp_prof (slots 0 .. 9: phases, slot 8 empty since the finish
-// pass took over the result row; 10 .. 13: event counts, 15: warps; 16 .. 20: the producer warp of scan_wp_batch_kernel).  32-bit sums
+// SM clock at the phase boundaries of a series, lane 0 adds its sums to g_wp_prof (slots 0 .. 9: phases, slot 8 the batch kernel's wait
+// for the previous result row's bulk store; 10 .. 13: event counts, 15: warps; 16 .. 20: the producer warp of scan_wp_batch_kernel).  32-bit sums
 // (a warp's share of one launch is far below 2^32 cycles) keep the register cost low.  Compiled out of the product build.
 #if defined(FILO_WP_PROF) && !defined(FILO_CUSIM)
 __device__ unsigned long long g_wp_prof[32];
@@ -593,9 +594,16 @@ __device__ __forceinline__ void wp_window_blocks(const double* V, uint8_t* wb, c
   __syncwarp();
 }
 
-// finish and store: lane-consecutive windows, 256 contiguous bytes per store instruction; O index of window lane + 32 m = oidx(lane) + 36 m
-template <int FN>
-__device__ __forceinline__ void wp_finish_store(double* __restrict__ out, int64_t s, const QueryParams& q, const double* O, const double* J,
+// finish and store: lane-consecutive windows, 256 contiguous bytes per store instruction; O index of window lane + 32 m = oidx(lane) + 36 m.
+// STAGE (scan_wp_batch_kernel): the finished row is written densely over O instead, window k at O[k + h] (h = 1 when the row starts at
+// 8 mod 16, so that O + 2h and the row's window h are both 16-byte aligned), and its span of windows [h, h + ((T - h) & ~1)) leaves as
+// one bulk store issued by lane 0; the window outside the span (0 or T - 1, at most one each) is stored directly.  The caller waits for
+// that store to have read O (wp_stage_wait) before anything writes V or O again.  Overwriting O in place is safe: a group of iterations
+// (4 x 32 windows, then 32) loads all its windows before any lane stores (__syncwarp in between: lanes may diverge), and a later group
+// starting at window G >= 32 loads from oidx(k) >= k + (k >> 3) > G, past every position G - 1 + h an earlier group wrote.  The trip
+// counts are warp-uniform for that barrier; only the last iteration has lanes with k >= T, which neither load nor store.
+template <int FN, bool STAGE = false>
+__device__ __forceinline__ void wp_finish_store(double* __restrict__ out, int64_t s, const QueryParams& q, double* O, const double* J,
                                                 const WpChunk* CD, int n, const WpPlan& M, const WpQuery& Q, int lane) {
   const double NaNv = __longlong_as_double(0x7ff8000000000000LL);
   const int psi = M.p_psi, Wr = M.p_Wr;
@@ -625,6 +633,45 @@ __device__ __forceinline__ void wp_finish_store(double* __restrict__ out, int64_
     if (code == WP_JUNC) jx >>= 8;
     return fin(o, code, js, k);
   };
+  if (STAGE) {
+    const int T = q.T;
+    double* row = out + (size_t)s * T;
+    const int h = (int)((reinterpret_cast<uintptr_t>(row) >> 3) & 1);
+    double* st = O + h + lane;
+    int k = lane, iters = (T + 31) >> 5;
+    int rest = iters > 16 ? iters - 16 : 0;
+    if (rest) iters = 16;
+    for (; iters >= 4; iters -= 4, st += 128, sp += 144, k += 128) {
+      const bool in3 = k + 96 < T;                             // (iterations before the last one have every window below T)
+      const double v0 = sp[0], v1 = sp[36], v2 = sp[72], v3 = in3 ? sp[108] : 0.0;
+      const double r0 = fin_m(v0, k), r1 = fin_m(v1, k + 32), r2 = fin_m(v2, k + 64), r3 = fin_m(v3, k + 96);
+      __syncwarp();
+      st[0] = r0; st[32] = r1; st[64] = r2; if (in3) st[96] = r3;
+    }
+    for (; iters > 0; --iters, st += 32, sp += 36, k += 32) {
+      const bool in = k < T;
+      const double r = fin_m(in ? *sp : 0.0, k);
+      __syncwarp();
+      if (in) *st = r;
+    }
+    for (; rest > 0; --rest, st += 32, sp += 36, k += 32) {     // windows from 512 on (multi-pass plans only)
+      const bool in = k < T;
+      uint32_t js;
+      const uint32_t code = wp_class(CD, n, k, js);
+      const double r = fin(in ? *sp : 0.0, code, js, k);
+      __syncwarp();
+      if (in) *st = r;
+    }
+    fence_async_smem();                                         // the row's writes, before the bulk store reads them
+    __syncwarp();
+    if (lane == 0) {
+      const int nb = (T - h) & ~1;
+      if (h) wp_store_result(row, O[1]);
+      if ((T - h) & 1) wp_store_result(row + T - 1, O[T - 1 + h]);
+      if (nb > 0) tma_store_1d(row + h, O + 2 * h, (uint32_t)nb * 8u);
+    }
+    return;
+  }
   int k = lane, iters = (q.T - lane + 31) >> 5;
   int rest = iters > 16 ? iters - 16 : 0;
   if (rest) iters = 16;
@@ -639,6 +686,11 @@ __device__ __forceinline__ void wp_finish_store(double* __restrict__ out, int64_
     const uint32_t code = wp_class(CD, n, k, js);
     wp_store_result(gp, fin(*sp, code, js, k));
   }
+}
+// the warp's previous result row (wp_finish_store<FN, true>) has been read out of O: V and O may be written again
+__device__ __forceinline__ void wp_stage_wait(int lane) {
+  if (lane == 0) tma_store_wait_read();
+  __syncwarp();
 }
 
 // per-series parts of the descriptors (lane c = chunk c): what the decode reads of each chunk
@@ -776,7 +828,7 @@ scan_wp_sum_kernel(const uint8_t* __restrict__ arena, const int64_t* __restrict_
     // ------------------------------------------------------------------------------------------------ finish and store
     wp_finish_store<FN>(out, s, q, O, J, CD, n, M, Q, lane);
     __syncwarp();
-    WPROF(7)                                               // finish and store (slot 8, the former result row, stays empty)
+    WPROF(7)                                               // finish and store (slot 8 stays empty in this kernel)
   }
   WPROF(9)
   WPROF_FLUSH
@@ -1004,6 +1056,8 @@ scan_wp_batch_kernel(const uint8_t* __restrict__ arena, const int64_t* __restric
     const bool any_raw = (flags & 2) != 0;
     __syncwarp();
     WPROF(3)                                               // per-series descriptors, scan counters
+    wp_stage_wait(lane);                                   // the previous row's bulk store has read O (O may sit on V)
+    WPROF(8)                                               // wait: previous result row's bulk store
     // ------------------------------------------------------------------------------------------------ decode
     // the record and the entry are dead once the fields are extracted: this series' share of the buffer is released
     auto rec_done = [&]() {
@@ -1029,13 +1083,14 @@ scan_wp_batch_kernel(const uint8_t* __restrict__ arena, const int64_t* __restric
     wp_window_blocks<FN>(V, wb, CD, L, M, Q, lane);
     WPROF(6)                                               // window blocks
     // ------------------------------------------------------------------------------------------------ finish and store
-    wp_finish_store<FN>(out, s, q, O, J, CD, n, M, Q, lane);
+    wp_finish_store<FN, true>(out, s, q, O, J, CD, n, M, Q, lane);
     __syncwarp();
-    WPROF(7)                                               // finish and store
+    WPROF(7)                                               // finish, stage and store
   }
   WPROF(9)
   WPROF_FLUSH
   if (lane == 0) {
+    tma_store_wait_all();
     if (rows_scanned | bytes_scanned) { atomicAdd(&d_counters[0], (unsigned long long)rows_scanned); atomicAdd(&d_counters[1], (unsigned long long)bytes_scanned); }
   }
 }

@@ -18,6 +18,12 @@ results), so 5 M rows read 18.8 GB and write 19.2 GB, as C2 does.  The shapes, t
               windows (2j - 1, 2j) in pairs, an even row windows (2j, 2j + 1) in pairs and window 480 alone
   warp_tma1   `warp_tma2` with one row in flight per warp, the next copy issued once the row is read (the C2 kernel's record stream)
   warp_tma1_v2, warp_tma2_v2   the two above with `copy_v2`'s 16-byte result stores
+  batch15     the C2 kernel's record stream: one CTA of 15 consumer warps and 1 producer warp per SM; the producer fetches batches of 15
+              consecutive rows into two buffers with one cp.async.bulk each (full / empty mbarriers); warp w takes row w of every batch,
+              releases the buffer once the row is read and stores its results with lane-consecutive 8-byte streaming stores
+  batch15_rowbulk  `batch15` with every result row staged densely in the warp's own shared memory (at offset h = 1 when the row starts
+              at 8 mod 16) and stored as one cp.async.bulk of its 16-byte-aligned span; the window outside the span (window 0 or 480)
+              is stored directly.  The warp waits for its previous row's store to have read the staging area before it reads the next row
 Prints the card's name, power limit and SM clocks beside each time and the rate against the 3.35 TB/s of the H100 SXM data sheet.
 The kernels are compiled with nvcc into a temporary directory."""
 import ctypes as C
@@ -30,7 +36,7 @@ import tempfile
 
 READ_B, WRITE_B = 3762, 3848
 SHAPES = ["copy", "read", "write", "pf_l2", "pair_v2", "warp_tma2", "bulk8_s3", "bulk4_s3x2", "copy_v2", "warp_tma1", "warp_tma1_v2",
-          "warp_tma2_v2"]
+          "warp_tma2_v2", "batch15", "batch15_rowbulk"]
 SRC = r"""
 #include <cstdint>
 #include <cuda_runtime.h>
@@ -51,6 +57,12 @@ __device__ __forceinline__ void bulk_load(void* d, const void* g, uint32_t bytes
   asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
                ::"r"(sa(d)), "l"(g), "r"(bytes), "r"(sa(b)) : "memory");
 }
+__device__ __forceinline__ void bar_init_n(uint64_t* b, uint32_t n) {
+  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(sa(b)), "r"(n) : "memory");
+  asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+}
+__device__ __forceinline__ void bar_arrive(uint64_t* b) { asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(sa(b)) : "memory"); }
 __device__ __forceinline__ void bar_wait(uint64_t* b, uint32_t parity) {
   uint32_t ok;
   do {
@@ -200,6 +212,62 @@ __global__ void __launch_bounds__(B * 32) c2_bulk(const uint4* __restrict__ src,
 }
 template <int B, int ST, int OST> constexpr int bulk_smem() { return ST * (((B * 3762 + 32 + 15) / 16) * 16) + OST * B * NT * 8 + 8 * ST; }
 
+// the C2 kernel's record stream (scan_wp_batch_kernel): batches of 15 consecutive rows, two batch buffers, warp 15 fetches them (one
+// cp.async.bulk per batch), consumer warp w takes row w of each batch and releases the buffer on `empty` once it has read the row.
+// ROWBULK: the result row is staged at stg[k + h] (h = 1 when the row starts at 8 mod 16) and its 16-byte-aligned span of windows
+// [h, h + ((481 - h) & ~1)) leaves as one cp.async.bulk store; the window outside it is stored directly
+constexpr int BT_B = 15, BT_NBUF = 2, BT_LB = ((BT_B * 3762 + 32 + 15) / 16) * 16, BT_SB = (((NT + 1) * 8 + 15) / 16) * 16;
+constexpr int batch_smem() { return BT_NBUF * BT_LB + BT_B * BT_SB + 2 * BT_NBUF * 8; }
+template <bool ROWBULK>
+__global__ void __launch_bounds__(512, 1) c2_batch(const uint4* __restrict__ src, double* __restrict__ dst, long long rows) {
+  extern __shared__ __align__(128) uint8_t sm[];
+  uint64_t* full = reinterpret_cast<uint64_t*>(sm + BT_NBUF * BT_LB + BT_B * BT_SB);
+  uint64_t* empty = full + BT_NBUF;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  auto first = [&](long long i) -> long long { return ((long long)blockIdx.x + i * gridDim.x) * BT_B; };
+  if (threadIdx.x == 0) for (int b = 0; b < BT_NBUF; ++b) { bar_init_n(full + b, 1); bar_init_n(empty + b, BT_B); }
+  __syncthreads();
+  if (warp == BT_B) {                                 // producer
+    if (lane == 0)
+      for (long long i = 0; first(i) < rows; ++i) {
+        const int b = (int)(i % BT_NBUF);
+        if (i >= BT_NBUF) bar_wait(empty + b, (uint32_t)(i / BT_NBUF - 1) & 1u);
+        const long long s1 = first(i) + BT_B < rows ? first(i) + BT_B : rows;
+        const long long a = first(i) * RB / 16, e = (s1 * RB + 15) / 16;
+        bulk_load(sm + b * BT_LB, src + a, (uint32_t)(e - a) * 16u, full + b);
+      }
+    return;
+  }
+  double* stg = reinterpret_cast<double*>(sm + BT_NBUF * BT_LB + warp * BT_SB);
+  for (long long i = 0;; ++i) {
+    const long long s = first(i) + warp;
+    if (s >= rows) break;
+    const int b = (int)(i % BT_NBUF);
+    bar_wait(full + b, (uint32_t)(i / BT_NBUF) & 1u);
+    if (ROWBULK && lane == 0) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");   // the previous row's store has read stg
+    const long long a = first(i) * RB / 16;
+    const uint4* r = reinterpret_cast<const uint4*>(sm + b * BT_LB);
+    unsigned long long acc = 0;
+    for (long long w = w_lo(s) + lane, w1 = w_lo(s + 1); w < w1; w += 32) acc ^= mix(r[w - a]);
+    __syncwarp();
+    if (lane == 0) bar_arrive(empty + b);
+    double* o = dst + s * NT;
+    if (!ROWBULK) { for (int k = lane; k < NT; k += 32) __stcs(o + k, (double)(acc + (unsigned long long)k + 1)); continue; }
+    const int h = (int)((reinterpret_cast<uintptr_t>(o) >> 3) & 1), nb = (NT - h) & ~1;
+    for (int k = lane; k < NT; k += 32) {
+      const double v = (double)(acc + (unsigned long long)k + 1);
+      if (k >= h && k < h + nb) stg[k + h] = v; else __stcs(o + k, v);
+    }
+    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+    __syncwarp();
+    if (lane == 0) {
+      asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;" ::"l"(o + h), "r"(sa(stg + 2 * h)), "r"((uint32_t)nb * 8u) : "memory");
+      asm volatile("cp.async.bulk.commit_group;" ::: "memory");
+    }
+  }
+  if (ROWBULK && lane == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
+}
+
 // shape k, one launch
 static int launch(int k, int sms, const uint4* src, double* dst, long long rows) {
   switch (k) {
@@ -215,6 +283,8 @@ static int launch(int k, int sms, const uint4* src, double* dst, long long rows)
     case 9: c2_warp_tma<1, false><<<sms, 640, 20 * (WT_BUF + 16)>>>(src, dst, rows); break;
     case 10: c2_warp_tma<1, true><<<sms, 640, 20 * (WT_BUF + 16)>>>(src, dst, rows); break;
     case 11: c2_warp_tma<2, true><<<sms, 640, 20 * (2 * WT_BUF + 16)>>>(src, dst, rows); break;
+    case 12: c2_batch<false><<<sms, 512, batch_smem()>>>(src, dst, rows); break;
+    case 13: c2_batch<true><<<sms, 512, batch_smem()>>>(src, dst, rows); break;
     default: return -1;
   }
   return 0;
@@ -237,6 +307,8 @@ extern "C" int c2_run(long long rows, int nshapes, int warmup, int reps, float* 
   cudaFuncSetAttribute(c2_warp_tma<1, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 20 * (WT_BUF + 16));
   cudaFuncSetAttribute(c2_bulk<8, 3, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, bulk_smem<8, 3, 2>());
   cudaFuncSetAttribute(c2_bulk<4, 3, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, bulk_smem<4, 3, 2>());
+  cudaFuncSetAttribute(c2_batch<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, batch_smem());
+  cudaFuncSetAttribute(c2_batch<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, batch_smem());
   const int sms = p.multiProcessorCount;
   for (int k = 0; k < nshapes; ++k) {
     check_out[k] = -1;

@@ -4,7 +4,8 @@
 (FILO_LIB_PATH: another profiling build, e.g. of an earlier commit.)
 Prints, per phase, the cycles a warp spends on one series (lane 0's SM clock, summed over warps and divided by the series the
 warps took up) and the share of the warp's time.  Warps of one SM run side by side: divide by the warps per SM for SM cycles.
-scan_wp_batch_kernel: "wait" is the wait for the entry and the record, "parse" the read of the entry; the producer warp's cycles
+scan_wp_batch_kernel: "wait" is the wait for the entry and the record, "parse" the read of the entry, and slot 8 the wait for the
+warp's previous result row to have left shared memory (its bulk store); the producer warp's cycles
 per batch follow (stalled on the empty barrier, offsets + copy issue + copy wait, header parse + entries)."""
 import ctypes as C
 import os
@@ -28,18 +29,16 @@ L.filo_debug_wp_prof(out.ctypes.data, 1)
 bench.main()
 L.filo_debug_wp_prof(out.ctypes.data, 0)
 names = ["wait: record (mbarrier)", "parse", "memo check (+ window plan on a miss)", "per-series descriptors, scan counters", "decode",
-         "zero rows", "window blocks", "finish and store (earlier: fix-up, gaps)", None, "loop head, declined series"]
-# slot 8: the result row of builds before the finish pass took it over; empty since
+         "zero rows", "window blocks", "finish and store (earlier: fix-up, gaps)", "wait: previous row's bulk store", "loop head, declined series"]
+# slot 8: scan_wp_batch_kernel's wait for its previous result row's bulk store (before the decode); zero for scan_wp_sum_kernel
 ns = float(out[10])
 tot = float(out[:10].sum())
 print("SUM kernel: %d consumer warps, %d series taken up, %d memo misses, %d declined by the plan, %d declined by the values"
       % (int(out[15]), int(ns), int(out[11]), int(out[12]), int(out[13])))
 print("  %-40s %10s %7s" % ("phase", "cyc/series", "share"))
 for i, n in enumerate(names):
-    if n is None:
-        if out[i] == 0:
-            continue
-        n = "result row (earlier builds)"
+    if i == 8 and out[i] == 0:
+        continue
     print("  %-40s %10.1f %6.1f %%" % (n, float(out[i]) / ns, 100.0 * float(out[i]) / tot))
 print("  %-40s %10.1f" % ("total", tot / ns))
 if out[20]:
