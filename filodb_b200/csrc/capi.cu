@@ -944,9 +944,15 @@ static int32_t query_device_impl(filo_ctx* ctx, const filo_table* t, int32_t fn,
     const WpSmem WL2 = wp_layout(t->max_rec_bytes, (uint32_t)t->max_rows, (uint32_t)t->max_chunks, (uint32_t)q.T, (uint32_t)wrows, alias, true);
     if (smem_cap / WL2.per_warp >= (size_t)WP_MAX_WARPS) {
       WL = WL2; WL.warps = WP_MAX_WARPS;
-      // that layout's record bytes as one CTA-wide stream: batches of consecutive records, a producer warp parses their headers
+      // that layout's record bytes as one CTA-wide stream: batches of consecutive records, a producer warp parses their headers.  Its
+      // layout adds the raw tail area behind the result row (no bytes for C2: the row and the area fit in V's region); where that does
+      // not fit, the table stays on scan_wp_sum_kernel with two record buffers per warp
       WB = wp_batch_layout(t->max_rec_bytes, (uint32_t)t->max_rows, (uint32_t)t->max_chunks, (uint32_t)q.T, (uint32_t)wrows, alias);
       use_wp_batch = WB.total <= smem_cap;
+      // the batch kernel's window blocks write finished windows over O right after the pass's reads of V: with O on V every plan must be
+      // one pass of at most 64 blocks
+      if (use_wp_batch && WB.W.alias && wp_max_items((uint32_t)t->max_chunks, (uint32_t)q.T, (uint32_t)wrows) > 64)
+        return fail(ctx, FILO_ERR_UNSUPPORTED, "scan_wp_batch_kernel: O on V with plans of more than one pass");
     }
     use_wp = WL.warps >= 4;
   }

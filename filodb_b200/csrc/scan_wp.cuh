@@ -21,8 +21,8 @@
 //            partial sum from each chunk's block list (the earlier chunk's in O, the later one's in J);
 //   finish   lane l = windows l + 32 m: one pass loads O (and J), finishes by the window's class (junction sums in chunk order, raw
 //            sums, windows without rows) and stores straight to the output: lane-consecutive streaming stores, 256 contiguous bytes
-//            per store instruction.  Nothing is written back to O.  scan_wp_batch_kernel instead writes the finished row over O and
-//            stores it with one bulk copy (wp_finish_store<FN, true>).
+//            per store instruction.  Nothing is written back to O.  scan_wp_batch_kernel instead stages the row densely in O: its window
+//            blocks write the finished windows there, a fix-up writes the rest, and one bulk copy stores the row (wp_finish_store<FN, true>).
 // Anything outside this fast path (irregular timestamps, DDV-long values, > 4 chunks, NaN / Inf / denormal / zero values, windows
 // shorter than 9 rows, windows over three chunks ...) is appended to the fallback list and answered by the v2 kernel into the same
 // output buffer, exactly as the tile kernel does.
@@ -351,9 +351,20 @@ __device__ __forceinline__ int wp_rows_in(const WpChunk& x, int k, int Wr) {    
   return hi - lo + 1;
 }
 
+// first slot of chunk c's raw tail partials in the raw tail area of scan_wp_batch_kernel: the chunks before it take (nblk - tb) blocks each
+__device__ __forceinline__ int wp_tail_base(const WpChunk* CD, int c) {
+  int t = 0;
+#pragma unroll
+  for (int x = 0; x < WP_MAXC - 1; ++x) if (x < c) t += CD[x].nblk - CD[x].tb;
+  return WP_R * t;
+}
+
 // window block `it` of the plan: V index of its first row, byte offset (inside the warp's region) of its first result slot, and
-// inf = (jEnd + 1) | raw << 4 | skew phase of the first slot << 5 | chunk << 8 | first window << 10, where slots 0 .. jEnd are stored
-__device__ __forceinline__ void wp_item(const WpChunk* CD, const WpSmem& L, int it, int items, int psi, int& pp, int& op, int& inf) {
+// inf = (jEnd + 1) | raw << 4 | skew phase of the first slot << 5 | chunk << 8 | first window << 10, where slots 0 .. jEnd are stored.
+// STAGE (scan_wp_batch_kernel): every block's slots are contiguous.  An own block's first slot is window k0 of the dense result row
+// (O[k0], the row's phase h is added by the window blocks), a raw tail block's is in the raw tail area at byte offset rt.
+template <bool STAGE = false>
+__device__ __forceinline__ void wp_item(const WpChunk* CD, const WpSmem& L, int it, int items, int psi, int& pp, int& op, int& inf, uint32_t rt = 0) {
   const bool active = it < items;
   int ci = 0;                                             // the last chunk with blocks whose blk0 <= it
   if (CD[1].nblk > 0 && it >= CD[1].blk0) ci = 1;
@@ -365,10 +376,11 @@ __device__ __forceinline__ void wp_item(const WpChunk* CD, const WpSmem& L, int 
   pp = ch.vidx0 + 9 * b;
   const bool tojz = b < ch.jzb;                           // raw sums to J (every slot of the block exists there)
   const bool raw = tojz || b >= ch.tb;
-  op = tojz ? (int)WP_OFF_J + 8 * (ch.joff + WP_R * b) : (int)L.out + 8 * (k0 + ((k0 + psi) >> 3));
+  if (STAGE) op = tojz ? (int)WP_OFF_J + 8 * (ch.joff + WP_R * b) : b >= ch.tb ? (int)rt + 8 * (wp_tail_base(CD, ci) + WP_R * (b - ch.tb)) : (int)L.out + 8 * k0;
+  else op = tojz ? (int)WP_OFF_J + 8 * (ch.joff + WP_R * b) : (int)L.out + 8 * (k0 + ((k0 + psi) >> 3));
   int jEnd = !active ? -1 : tojz ? WP_R - 1 : ch.kT1 - k0;
   if (jEnd > WP_R - 1) jEnd = WP_R - 1;
-  const int ot = tojz ? 0 : (k0 + psi) & 7;               // slots j with ot + j >= 8 sit one pad slot further
+  const int ot = tojz || STAGE ? 0 : (k0 + psi) & 7;      // slots j with ot + j >= 8 sit one pad slot further
   inf = (jEnd + 1) | ((raw ? 1 : 0) << 4) | (ot << 5) | (ci << 8) | (k0 << 10);
 }
 
@@ -401,9 +413,12 @@ struct WpPlan {
 };
 
 // Memo check and, on a miss, the window plan of a regular series (lane c = chunk c, the fields wp_parse gives).  Clears `regular` when the
-// plan declines the series.  Returns true on a memo miss.
+// plan declines the series.  Returns true on a memo miss.  STAGE: the work items of scan_wp_batch_kernel (wp_item<true>), raw tail area at
+// byte offset rt with rtcap doubles.
+template <bool STAGE = false>
 __device__ __forceinline__ bool wp_plan_series(WpPlan& M, bool& regular, bool have, int n, int64_t init, int64_t end_time, int nrows, int vwire,
-                                               int grp_base, int ngroups, const QueryParams& q, const WpSmem& L, const WpQuery& Q, WpChunk* CD, int lane) {
+                                               int grp_base, int ngroups, const QueryParams& q, const WpSmem& L, const WpQuery& Q, WpChunk* CD, int lane,
+                                               uint32_t rt = 0, uint32_t rtcap = 0) {
   const unsigned FULL = 0xffffffffu;
   const int c = lane;
   const bool samec = !(c < n) || (init == M.m_init && nrows == M.m_nrows && end_time == M.m_end && vwire == M.m_wire);
@@ -444,6 +459,11 @@ __device__ __forceinline__ bool wp_plan_series(WpPlan& M, bool& regular, bool ha
       const int a0 = __shfl_sync(FULL, z, 0), a1 = __shfl_sync(FULL, z, 1), a2 = __shfl_sync(FULL, z, 2), a3 = __shfl_sync(FULL, z, 3);
       joff = (c > 0 ? a0 : 0) + (c > 1 ? a1 : 0) + (c > 2 ? a2 : 0); jtot = a0 + a1 + a2 + a3; }
     if ((uint32_t)jtot > L.jcap) okp = false;
+    if (STAGE) {                                            // (wp_batch_layout sizes the area for every plan: this never declines)
+      const int t = nblk - tb;
+      const int a0 = __shfl_sync(FULL, t, 0), a1 = __shfl_sync(FULL, t, 1), a2 = __shfl_sync(FULL, t, 2);
+      if ((uint32_t)(WP_R * (a0 + a1 + a2)) > rtcap) okp = false;
+    }
     if (L.alias && items > 64) okp = false;                 // O takes V's place: every block is summed before the first result is stored
     // row positions: chunk after chunk, Wr .. Wr + 7 zero rows in between, every chunk's block 0 at a multiple of 8
     const int fr = touch ? (int)(s0 + kT0) : 0;              // first row of block 0 (may be negative: zero rows in front)
@@ -518,7 +538,7 @@ __device__ __forceinline__ bool wp_plan_series(WpPlan& M, bool& regular, bool ha
           M.dd_inf[jj] = (active ? 1 : 0) | (ci << 1) | ((pq & 7) << 3) | (g << 8);      // active, chunk, skew phase of the first row, group in chunk
         }
 #pragma unroll
-        for (int X = 0; X < 2; ++X) wp_item(CD, L, X * 32 + lane, items, M.p_psi, M.wi_pp[X], M.wi_op[X], M.wi_inf[X]);
+        for (int X = 0; X < 2; ++X) wp_item<STAGE>(CD, L, X * 32 + lane, items, M.p_psi, M.wi_pp[X], M.wi_op[X], M.wi_inf[X], rt);
       }
       M.m_ok = true;
     }
@@ -541,10 +561,19 @@ __device__ __forceinline__ void wp_zero_rows(double* V, const WpChunk* CD, int n
   }
 }
 
-// window blocks of a decoded series: two items per lane, 64 per pass, results (finished or raw) into O and J of the warp's region wb
-template <int FN>
+// window blocks of a decoded series: two items per lane, 64 per pass, results (finished or raw) into O and J of the warp's region wb.
+// STAGE (scan_wp_batch_kernel): an own block writes its finished windows k straight into the dense result row, O[k + h] (h: the row's
+// phase, see wp_finish_store); raw tail blocks write to the raw tail area, head-share blocks to J.  With O on V the single __syncwarp
+// between a pass's row loads and its stores separates the last read of V from the first write over it: O sits on V only when every
+// plan is one pass of at most 64 items (WpSmem::alias; the plan declines longer ones, the host asserts it).  A block's 8 slots are
+// stored in an order rotated by r = 4 ((lane >> 1) & 1): lane l's block starts 8 l windows on, so with the same slot order the lanes of
+// one parity would all hit one bank pair (16 wavefronts per 8-byte store).  Rotated, step j stores slot (j + r) & 7 and each parity
+// hits two bank pairs: 8 wavefronts per store, 64 per 32 items, for one stage of selects.  (Rotations over 4 and 8 slot orders, 32
+// and 16 wavefronts per 32 items for two and three stages of selects, ran C2 slower on an H100: its per-series path is bound by
+// issued instructions more than by shared-memory wavefronts.  Without rotation it ran slower than with the finish pass.)
+template <int FN, bool STAGE = false>
 __device__ __forceinline__ void wp_window_blocks(const double* V, uint8_t* wb, const WpChunk* CD, const WpSmem& L, const WpPlan& M, const WpQuery& Q,
-                                                 int lane) {
+                                                 int lane, int h = 0, uint32_t rt = 0) {
   const int psi = M.p_psi;
   const int Wr = M.p_Wr;
   for (int it0 = 0; it0 < M.p_items; it0 += 64) {
@@ -552,13 +581,14 @@ __device__ __forceinline__ void wp_window_blocks(const double* V, uint8_t* wb, c
 #pragma unroll
     for (int X = 0; X < 2; ++X) {
       if (it0 == 0) { ipp[X] = M.wi_pp[X]; iop[X] = M.wi_op[X]; iinf[X] = M.wi_inf[X]; }
-      else wp_item(CD, L, it0 + X * 32 + lane, M.p_items, psi, ipp[X], iop[X], iinf[X]);
+      else wp_item<STAGE>(CD, L, it0 + X * 32 + lane, M.p_items, psi, ipp[X], iop[X], iinf[X], rt);
     }
     const double* pp[2]; double* op[2]; int jEnd[2], ot[2]; bool rawm[2];
 #pragma unroll
     for (int X = 0; X < 2; ++X) {
       pp[X] = V + ipp[X]; op[X] = reinterpret_cast<double*>(wb + iop[X]);
       jEnd[X] = (iinf[X] & 15) - 1; rawm[X] = (iinf[X] >> 4) & 1; ot[X] = (iinf[X] >> 5) & 7;
+      if (STAGE && !rawm[X]) op[X] += h;
     }
     double a[WP_R], bb[WP_R];
     wp_block_pair(pp[0], pp[1], Wr, a, bb);
@@ -580,7 +610,20 @@ __device__ __forceinline__ void wp_window_blocks(const double* V, uint8_t* wb, c
         if (X) bb[j] = fin; else a[j] = fin;
       }
     }
-    if (M.p_oal) {                                      // every block starts on O's 9-word grid: constant store offsets
+    if (STAGE) {
+      const int r = 4 * ((lane >> 1) & 1);
+#pragma unroll
+      for (int X = 0; X < 2; ++X) {
+        double (&v)[WP_R] = X ? bb : a;
+        double t[WP_R];                                   // v[j] = slot (j + r) & 7, by selects (no dynamic register index)
+#pragma unroll
+        for (int j = 0; j < WP_R; ++j) t[j] = r ? v[(j + 4) & 7] : v[j];
+#pragma unroll
+        for (int j = 0; j < WP_R; ++j) v[j] = t[j];
+#pragma unroll
+        for (int j = 0; j < WP_R; ++j) { const int sj = (j + r) & 7; if (sj <= jEnd[X]) op[X][sj] = v[j]; }
+      }
+    } else if (M.p_oal) {                               // every block starts on O's 9-word grid: constant store offsets
 #pragma unroll
       for (int j = 0; j < WP_R; ++j) { if (j <= jEnd[0]) op[0][j] = a[j]; if (j <= jEnd[1]) op[1][j] = bb[j]; }
     } else {
@@ -595,16 +638,17 @@ __device__ __forceinline__ void wp_window_blocks(const double* V, uint8_t* wb, c
 }
 
 // finish and store: lane-consecutive windows, 256 contiguous bytes per store instruction; O index of window lane + 32 m = oidx(lane) + 36 m.
-// STAGE (scan_wp_batch_kernel): the finished row is written densely over O instead, window k at O[k + h] (h = 1 when the row starts at
-// 8 mod 16, so that O + 2h and the row's window h are both 16-byte aligned), and its span of windows [h, h + ((T - h) & ~1)) leaves as
-// one bulk store issued by lane 0; the window outside the span (0 or T - 1, at most one each) is stored directly.  The caller waits for
-// that store to have read O (wp_stage_wait) before anything writes V or O again.  Overwriting O in place is safe: a group of iterations
-// (4 x 32 windows, then 32) loads all its windows before any lane stores (__syncwarp in between: lanes may diverge), and a later group
-// starting at window G >= 32 loads from oidx(k) >= k + (k >> 3) > G, past every position G - 1 + h an earlier group wrote.  The trip
-// counts are warp-uniform for that barrier; only the last iteration has lanes with k >= T, which neither load nor store.
+// STAGE (scan_wp_batch_kernel): the row is dense in O, window k at O[k + h] (h = 1 when the row starts at 8 mod 16, so that O + 2h and
+// the row's window h are both 16-byte aligned).  The window blocks (wp_window_blocks<FN, true>) already wrote every WP_FINAL window there;
+// this fix-up writes the others: junction sums (the earlier chunk's raw partial from the raw tail area RT first, then J), raw sums of own
+// windows from RT, NaN for windows without rows.  Each window is written by one lane, and nothing the fix-up reads is written here.
+// Then the row's span of windows [h, h + ((T - h) & ~1)) leaves as one bulk store issued by lane 0; the window outside the span (0 or
+// T - 1, at most one each) is stored directly.  The caller waits for that store to have read O (wp_stage_wait) before anything writes V
+// or O again.
 template <int FN, bool STAGE = false>
 __device__ __forceinline__ void wp_finish_store(double* __restrict__ out, int64_t s, const QueryParams& q, double* O, const double* J,
-                                                const WpChunk* CD, int n, const WpPlan& M, const WpQuery& Q, int lane) {
+                                                const WpChunk* CD, int n, const WpPlan& M, const WpQuery& Q, int lane, const double* RT = nullptr,
+                                                int h = 0) {
   const double NaNv = __longlong_as_double(0x7ff8000000000000LL);
   const int psi = M.p_psi, Wr = M.p_Wr;
   auto oidx = [&](int k) -> int { return k + ((k + psi) >> 3); };
@@ -636,31 +680,28 @@ __device__ __forceinline__ void wp_finish_store(double* __restrict__ out, int64_
   if (STAGE) {
     const int T = q.T;
     double* row = out + (size_t)s * T;
-    const int h = (int)((reinterpret_cast<uintptr_t>(row) >> 3) & 1);
-    double* st = O + h + lane;
-    int k = lane, iters = (T + 31) >> 5;
-    int rest = iters > 16 ? iters - 16 : 0;
-    if (rest) iters = 16;
-    for (; iters >= 4; iters -= 4, st += 128, sp += 144, k += 128) {
-      const bool in3 = k + 96 < T;                             // (iterations before the last one have every window below T)
-      const double v0 = sp[0], v1 = sp[36], v2 = sp[72], v3 = in3 ? sp[108] : 0.0;
-      const double r0 = fin_m(v0, k), r1 = fin_m(v1, k + 32), r2 = fin_m(v2, k + 64), r3 = fin_m(v3, k + 96);
-      __syncwarp();
-      st[0] = r0; st[32] = r1; st[64] = r2; if (in3) st[96] = r3;
+    // the raw partial of chunk c for window k, from the raw tail area
+    auto tail = [&](int c, int k) -> double { return RT[wp_tail_base(CD, c) + k - CD[c].kT0 - WP_R * CD[c].tb]; };
+    auto fix = [&](uint32_t code, uint32_t js, int k) {
+      double o = 0.0;
+      if (code == WP_RAWFIN) o = tail(wp_chunk_of(CD, n, k), k);
+      else if (code == WP_JUNC && (js & 128u)) o = tail(wp_chunk_of(CD, n, k) - 1, k);
+      O[k + h] = fin(o, code, js, k);
+    };
+    // windows lane + 32 m, m < 16, that the window blocks left unfinished: class from the plan, J slot from the cursor
+    uint32_t nf = (cls | (cls >> 1)) & 0x55555555u;
+    while (nf) {
+      const int b = __ffs((int)nf) - 1;
+      nf &= nf - 1;
+      const uint32_t code = (cls >> b) & 3u;
+      uint32_t js = 0;
+      if (code == WP_JUNC) { js = (uint32_t)jx & 0xffu; jx >>= 8; }
+      fix(code, js, lane + 16 * b);
     }
-    for (; iters > 0; --iters, st += 32, sp += 36, k += 32) {
-      const bool in = k < T;
-      const double r = fin_m(in ? *sp : 0.0, k);
-      __syncwarp();
-      if (in) *st = r;
-    }
-    for (; rest > 0; --rest, st += 32, sp += 36, k += 32) {     // windows from 512 on (multi-pass plans only)
-      const bool in = k < T;
+    for (int k = lane + 512; k < T; k += 32) {                  // windows from 512 on (multi-pass plans only)
       uint32_t js;
       const uint32_t code = wp_class(CD, n, k, js);
-      const double r = fin(in ? *sp : 0.0, code, js, k);
-      __syncwarp();
-      if (in) *st = r;
+      if (code != WP_FINAL) fix(code, js, k);
     }
     fence_async_smem();                                         // the row's writes, before the bulk store reads them
     __syncwarp();
@@ -1038,7 +1079,7 @@ scan_wp_batch_kernel(const uint8_t* __restrict__ arena, const int64_t* __restric
     }
     const int vwire = wire & 0xffff;
     WPROF(1)                                               // entry
-    if (wp_plan_series(M, regular, have, n, init, end_time, nrows, vwire, grp_base, e.ngroups, q, L, Q, CD, lane)) { WPROF_COUNT(11) }
+    if (wp_plan_series<true>(M, regular, have, n, init, end_time, nrows, vwire, grp_base, e.ngroups, q, L, Q, CD, lane, BL.rt, BL.rtcap)) { WPROF_COUNT(11) }
     WPROF(2)                                               // memo check (+ window plan on a miss)
     if (!regular) {
       // declined: the v2 kernel answers this series
@@ -1080,12 +1121,14 @@ scan_wp_batch_kernel(const uint8_t* __restrict__ arena, const int64_t* __restric
     if (lane == 0) { rows_scanned += cnt_rows; bytes_scanned += cnt_bytes; }
     __syncwarp();
     // ------------------------------------------------------------------------------------------------ windows
-    wp_window_blocks<FN>(V, wb, CD, L, M, Q, lane);
-    WPROF(6)                                               // window blocks
-    // ------------------------------------------------------------------------------------------------ finish and store
-    wp_finish_store<FN, true>(out, s, q, O, J, CD, n, M, Q, lane);
+    // the row's phase: h = 1 when out + s T is 8 mod 16 (filo_query_device writes into a caller's buffer)
+    const int h = (int)((reinterpret_cast<uintptr_t>(out + s * q.T) >> 3) & 1);
+    wp_window_blocks<FN, true>(V, wb, CD, L, M, Q, lane, h, BL.rt);
+    WPROF(6)                                               // window blocks (finished windows into the dense row)
+    // ------------------------------------------------------------------------------------------------ fix-up and store
+    wp_finish_store<FN, true>(out, s, q, O, J, CD, n, M, Q, lane, reinterpret_cast<const double*>(wb + BL.rt), h);
     __syncwarp();
-    WPROF(7)                                               // finish, stage and store
+    WPROF(7)                                               // fix-up and store
   }
   WPROF(9)
   WPROF_FLUSH

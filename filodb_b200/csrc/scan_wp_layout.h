@@ -92,6 +92,8 @@ struct WpBatchSmem {                   // byte offsets inside the CTA's shared m
   uint32_t ent;                        // WpEntry[nbuf][B]
   uint32_t bars;                       // mbarriers full[nbuf], parsed[nbuf], empty[nbuf]
   uint32_t total;                      // bytes per CTA
+  uint32_t rt, rtcap;                  // raw tail area of a warp's region (byte offset, doubles): the raw sums of every chunk's blocks from tb on,
+                                       // behind the dense result row in O (windows [0, T) at O[h .. T - 1 + h], h <= 1)
 };
 FILO_HD inline WpBatchSmem wp_batch_layout(uint32_t max_rec_bytes, uint32_t max_rows, uint32_t max_chunks, uint32_t T, uint32_t wrows, bool alias,
                                            uint32_t B = WP_BATCH_SERIES, uint32_t nbuf = WP_BATCH_BUFS, uint32_t consumers = WP_BATCH_WARPS - 1) {
@@ -99,6 +101,14 @@ FILO_HD inline WpBatchSmem wp_batch_layout(uint32_t max_rec_bytes, uint32_t max_
   WpSmem L = wp_layout(max_rec_bytes, max_rows, max_chunks, T, wrows, alias);
   const uint32_t shift = L.vals - WP_OFF_REC;                                 // the record buffer leaves the warp's region
   L.vals -= shift; L.out -= shift; L.per_warp -= shift; L.rec = 0;
+  // raw tail area: a chunk followed by another leaves raw sums in its blocks [tb, nblk), at most (Wr - 1) / 8 + 2 blocks with
+  // Wr <= wrows - 1 (at most Wr windows take rows from both chunks).  O's region grows only where T + 1 + rtcap exceed it; vcap (what
+  // the plan checks V against) stays as it is
+  const uint32_t mc = max_chunks < (uint32_t)WP_MAXC ? max_chunks : (uint32_t)WP_MAXC;
+  S.rtcap = mc > 1 ? (uint32_t)WP_R * (mc - 1) * ((wrows + 14) / 8) : 0;
+  S.rt = L.out + 8 * (T + 1);
+  { const uint32_t oreg = alias ? L.vcap : L.ocap, need = T + 1 + S.rtcap;
+    L.per_warp = align_up(L.out + 8 * (oreg > need ? oreg : need), 16); }
   S.consumers = consumers;
   L.warps = S.consumers;
   S.W = L; S.B = B; S.nbuf = nbuf;

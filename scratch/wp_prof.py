@@ -29,7 +29,7 @@ L.filo_debug_wp_prof(out.ctypes.data, 1)
 bench.main()
 L.filo_debug_wp_prof(out.ctypes.data, 0)
 names = ["wait: record (mbarrier)", "parse", "memo check (+ window plan on a miss)", "per-series descriptors, scan counters", "decode",
-         "zero rows", "window blocks", "finish and store (earlier: fix-up, gaps)", "wait: previous row's bulk store", "loop head, declined series"]
+         "zero rows", "window blocks", "finish and store (batch kernel: fix-up and store)", "wait: previous row's bulk store", "loop head, declined series"]
 # slot 8: scan_wp_batch_kernel's wait for its previous result row's bulk store (before the decode); zero for scan_wp_sum_kernel
 ns = float(out[10])
 tot = float(out[:10].sum())
