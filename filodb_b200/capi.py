@@ -18,7 +18,7 @@ OK, ERR_INVALID_ARG, ERR_CUDA, ERR_CORRUPT_VECTOR, ERR_UNSUPPORTED, ERR_QUERY_LI
 
 EXPORTS = ["filo_ctx_create", "filo_ctx_destroy", "filo_ctx_set_fn_args", "filo_ctx_check", "filo_last_error", "filo_load_series", "filo_table_append", "filo_synth_table", "filo_encode_table", "filo_encode_hist_table", "filo_synth_hist_table",
            "filo_table_set_groups", "filo_table_get_info", "filo_table_read_record", "filo_table_read_arena", "filo_table_free",
-           "filo_num_windows", "filo_query", "filo_query_device", "filo_scan_series", "filo_query_hist", "filo_query_hist_device", "filo_merge_hist_partials", "filo_query_avg_sum_count", "filo_host_register", "filo_host_unregister", "filo_present_partials",
+           "filo_num_windows", "filo_query", "filo_query_device", "filo_scan_series", "filo_query_hist", "filo_query_hist_device", "filo_merge_hist_partials", "filo_merge_topk_partials", "filo_query_avg_sum_count", "filo_host_register", "filo_host_unregister", "filo_present_partials",
            "filo_result_max_containers", "filo_encode_result_device", "filo_encode_result"]
 
 
@@ -106,6 +106,8 @@ def _sig(L):
     L.filo_query_hist_device.argtypes = [vp, vp, i32, i64, i64, i64, i64, i32, C.c_double, vp, vp, vp, C.POINTER(Stats)]
     L.filo_merge_hist_partials.restype = i32
     L.filo_merge_hist_partials.argtypes = [vp, vp, i32, i32, C.c_double, vp, vp, vp, vp]
+    L.filo_merge_topk_partials.restype = i32
+    L.filo_merge_topk_partials.argtypes = [vp, i32, i32, i32, i32, i32, vp, vp, vp, vp, vp]
     L.filo_query_avg_sum_count.restype = i32; L.filo_query_avg_sum_count.argtypes = [vp, vp, vp, i64, i64, i64, i64, vp, C.POINTER(Stats)]
     L.filo_host_register.restype = i32; L.filo_host_register.argtypes = [vp, vp, i64]
     L.filo_host_unregister.restype = i32; L.filo_host_unregister.argtypes = [vp, vp]
@@ -416,6 +418,13 @@ class Context:
         self._check(lib().filo_merge_hist_partials(self.h, table.h, n_parts, n_windows, float("nan") if quantile is None else float(quantile),
                                                    C.c_void_p(d_parts) if d_parts else None, C.c_void_p(d_out_values) if d_out_values else None,
                                                    C.c_void_p(d_out_quantile) if d_out_quantile else None, C.c_void_p(stream) if stream else None))
+
+    def merge_topk_partials(self, aggr, k, n_parts, n_groups, n_windows, d_part_values, d_part_ids, d_out_values, d_out_ids, stream=0):
+        """filo_merge_topk_partials: the k best candidates per (group, window) of n_parts topk / bottomk outputs [n_parts, G, T, k] (device
+        addresses, ids global series ordinals) into values / ids [G, T, k], in the form filo_query_device writes them."""
+        ptr = lambda a: C.c_void_p(a) if a else None
+        self._check(lib().filo_merge_topk_partials(self.h, aggr, k, n_parts, n_groups, n_windows, ptr(d_part_values), ptr(d_part_ids),
+                                                   ptr(d_out_values), ptr(d_out_ids), ptr(stream)))
 
     def present_partials(self, aggr, n, d_values, d_counts, d_out, stream=0):
         self._check(lib().filo_present_partials(self.h, aggr, n, C.c_void_p(d_values), C.c_void_p(d_counts), C.c_void_p(d_out),

@@ -1598,6 +1598,20 @@ extern "C" int32_t filo_merge_hist_partials(filo_ctx* ctx, const filo_table* t, 
   return FILO_OK;
 }
 
+extern "C" int32_t filo_merge_topk_partials(filo_ctx* ctx, int32_t agg, int32_t k, int32_t n_parts, int32_t n_groups, int32_t n_windows,
+                                            const void* d_part_values, const void* d_part_ids, void* d_out_values, void* d_out_ids, void* cuda_stream) {
+  if (!ctx || !d_part_values || !d_part_ids || !d_out_values || !d_out_ids) return fail(ctx, FILO_ERR_INVALID_ARG, "filo_merge_topk_partials: null argument");
+  if (agg != FILO_AGG_TOPK && agg != FILO_AGG_BOTTOMK) return fail(ctx, FILO_ERR_INVALID_ARG, "filo_merge_topk_partials: the operator must be topk or bottomk");
+  if (k < 1 || k > FILO_MAX_TOPK) return fail(ctx, FILO_ERR_INVALID_ARG, "topk/bottomk k must be in [1, 32]");
+  if (n_parts < 1 || n_groups < 1 || n_windows < 1) return fail(ctx, FILO_ERR_INVALID_ARG, "filo_merge_topk_partials: n_parts, n_groups and n_windows must be >= 1");
+  CUDA_TRY(ctx, cudaSetDevice(ctx->device));
+  { const int32_t prc = poll_async_errors(ctx, false); if (prc != FILO_OK) return prc; }      // e.g. the query that produced a part failed
+  cudaStream_t s = cuda_stream ? (cudaStream_t)cuda_stream : ctx->stream;
+  CUDA_TRY(ctx, launch_topk_merge_parts((const double*)d_part_values, (const int64_t*)d_part_ids, n_parts, (int64_t)n_groups * n_windows, k,
+                                        agg == FILO_AGG_BOTTOMK ? 1 : 0, (double*)d_out_values, (int64_t*)d_out_ids, s));
+  return FILO_OK;
+}
+
 extern "C" int32_t filo_present_partials(filo_ctx* ctx, int32_t agg, int64_t n, void* d_values, void* d_counts, void* d_out, void* cuda_stream) {
   if (!ctx || !d_values || !d_counts || !d_out || n < 0) return fail(ctx, FILO_ERR_INVALID_ARG, "filo_present_partials: bad argument");
   CUDA_TRY(ctx, cudaSetDevice(ctx->device));

@@ -51,6 +51,9 @@ cudaError_t launch_merge_partials(const double* pval, const uint32_t* pcnt, cons
 cudaError_t launch_present(int agg_op, int64_t n, const double* vals, const int64_t* cnts, double* out, cudaStream_t s);
 cudaError_t launch_topk(const double* per_series, const int32_t* order, const int64_t* group_start, int n_groups, int T, int k, int bottom,
                         double* out_val, int64_t* out_id, cudaStream_t s);
+// merge of n_parts topk_kernel outputs [n_parts][n_cells][k] (ids global series ordinals, -1 = empty) into [n_cells][k]
+cudaError_t launch_topk_merge_parts(const double* part_val, const int64_t* part_id, int n_parts, int64_t n_cells, int k, int bottom,
+                                    double* out_val, int64_t* out_id, cudaStream_t s);
 struct WpSmem;
 cudaError_t launch_scan_wp(const ScanLaunch& L, double* out, const WpSmem& W, int64_t* fallback_list, unsigned long long* fallback_count);
 struct WpBatchSmem;

@@ -260,6 +260,73 @@ __global__ void topk_kernel(const double* __restrict__ per_series, const int32_t
   }
 }
 
+// topk / bottomk across GPUs (ReduceAggregateExec over TopBottomKRowAggregator rows): n_parts outputs of topk_kernel, ids mapped to
+// global series ordinals, [n_parts][n_cells][k] in rank order.  (value, ordinal) is a strict total order: among equal values (==, so
+// +0.0 ties -0.0) the smaller ordinal is better.  An empty slot is one whose id is -1 (±DBL_MAX padding is also a real value); a NaN value,
+// which topk_kernel never writes with an id, is skipped like one, so that the order stays total.
+__device__ __forceinline__ bool topk_better(double a, int64_t ai, double b, int64_t bi, int bottom) {
+  if (bi < 0) return ai >= 0;                                         // any candidate beats an empty slot
+  if (ai < 0) return false;
+  if (a != b) return bottom ? a < b : a > b;
+  return ai < bi;
+}
+// folds slot (v, id) into (cv, cid) when it lies strictly below the bound (tv, tid) (tid < 0: no bound)
+__device__ __forceinline__ void topk_fold_below(double v, int64_t id, double tv, int64_t tid, int bottom, double& cv, int64_t& cid) {
+  if (id < 0 || v != v) return;
+  if (tid >= 0 && !topk_better(tv, tid, v, id, bottom)) return;      // emitted already
+  if (topk_better(v, id, cv, cid, bottom)) { cv = v; cid = id; }
+}
+// warp-wide arg-best: every lane ends with the best (v, id) of the warp, a non-empty one whenever any lane holds one
+__device__ __forceinline__ void topk_warp_best(double& v, int64_t& id, int bottom) {
+  for (int o = 16; o > 0; o >>= 1) {
+    const double ov = __shfl_xor_sync(0xffffffffu, v, o);
+    const int64_t oi = __shfl_xor_sync(0xffffffffu, id, o);
+    if (topk_better(ov, oi, v, id, bottom)) { v = ov; id = oi; }
+  }
+}
+// One warp per (group, window) cell: a W-way merge.  Lane l holds the best candidate of parts l, l + 32, ... not emitted yet; k rounds
+// of a warp-wide arg-best emit the candidates best first.  The elements emitted are exactly those at or above the last winner, so a
+// lane's next candidate is the best slot of its parts strictly below the winner: after each round the whole warp reads the winning
+// lane's parts (lane j reads slot j) and reduces them.  Nothing depends on the order of the slots inside a part, so the result is the k
+// best of all non-empty slots whatever local -> global map produced the ordinals.  Round r's winner stays in lane r, and the cell is
+// written the way topk_kernel writes one: worst first, then the padding.  Value bits pass through unchanged.
+__global__ void topk_merge_parts_kernel(const double* __restrict__ pv, const int64_t* __restrict__ pid, int n_parts, int64_t n_cells, int kk,
+                                        int bottom, double* __restrict__ out_val, int64_t* __restrict__ out_id) {
+  const int64_t cell = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  if (cell >= n_cells) return;                                        // warp-uniform
+  const int lane = threadIdx.x & 31;
+  double cv = 0.0; int64_t cid = -1;
+  for (int p = lane; p < n_parts; p += 32) {
+    const size_t base = ((size_t)p * n_cells + cell) * kk;
+    for (int s = 0; s < kk; ++s) topk_fold_below(pv[base + s], pid[base + s], 0.0, -1, bottom, cv, cid);
+  }
+  double rv = 0.0; int64_t rid = -1;
+  int m = 0;
+  for (; m < kk; ++m) {
+    double bv = cv; int64_t bi = cid;
+    topk_warp_best(bv, bi, bottom);
+    if (bi < 0) break;                                                // every part is exhausted (uniform: see topk_warp_best)
+    if (lane == m) { rv = bv; rid = bi; }
+    // the lane the winner came from (the winner is some lane's candidate, so the ballot is never empty; the lowest such lane)
+    const int wl = __ffs(__ballot_sync(0xffffffffu, cid >= 0 && cid == bi)) - 1;
+    double nv = 0.0; int64_t ni = -1;
+    for (int p = wl; p < n_parts; p += 32) {
+      const size_t i = ((size_t)p * n_cells + cell) * kk + lane;
+      if (lane < kk) topk_fold_below(pv[i], pid[i], bv, bi, bottom, nv, ni);
+    }
+    topk_warp_best(nv, ni, bottom);
+    if (lane == wl) { cv = nv; cid = ni; }
+  }
+  const int src = lane < m ? m - 1 - lane : lane;
+  const double wv = __shfl_sync(0xffffffffu, rv, src);
+  const int64_t wi = __shfl_sync(0xffffffffu, rid, src);
+  if (lane < kk) {
+    const size_t o = (size_t)cell * kk + lane;
+    if (lane < m) { out_val[o] = wv; out_id[o] = wi; }
+    else { out_val[o] = bottom ? 1.7976931348623157e308 : -1.7976931348623157e308; out_id[o] = -1; }
+  }
+}
+
 // ---------------------------------------------------------------------------------------------------------------
 // group bookkeeping (device side, so that synthetic tables never leave the GPU)
 // ---------------------------------------------------------------------------------------------------------------
@@ -633,6 +700,11 @@ cudaError_t launch_topk(const double* per_series, const int32_t* order, const in
                         double* out_val, int64_t* out_id, cudaStream_t s) {
   const int64_t n = (int64_t)n_groups * T;
   topk_kernel<<<(unsigned)((n + 127) / 128), 128, 0, s>>>(per_series, order, group_start, n_groups, T, k, bottom, out_val, out_id);
+  return cudaGetLastError();
+}
+cudaError_t launch_topk_merge_parts(const double* part_val, const int64_t* part_id, int n_parts, int64_t n_cells, int k, int bottom,
+                                    double* out_val, int64_t* out_id, cudaStream_t s) {
+  topk_merge_parts_kernel<<<(unsigned)((n_cells + 7) / 8), 256, 0, s>>>(part_val, part_id, n_parts, n_cells, k, bottom, out_val, out_id);
   return cudaGetLastError();
 }
 cudaError_t launch_iota(int32_t* a, int64_t n, cudaStream_t s) {

@@ -4,7 +4,8 @@ One process per GPU.  Series are independent until the across-series aggregate (
 collective for per-series queries; aggregates merge `[G x T]` partials (FILO_Q_PARTIAL form, include/filo_b200.h) with
 one all-reduce, the role `LocalPartitionReduceAggregateExec` + `RowAggregator.reduceAggregate` play in the reference
 (query/exec/AggrOverRangeVectors.scala:119-182; aggregator/*RowAggregator.scala).  Histogram sums are gathered instead
-(gather_hist_partials) and folded in rank order on the device by filo_merge_hist_partials.
+(gather_hist_partials) and folded in rank order on the device by filo_merge_hist_partials; topk / bottomk candidates are mapped
+to global series ordinals (topk_ids_to_global), gathered (gather_topk_partials) and selected again by filo_merge_topk_partials.
 
 Works on CUDA tensors over NCCL (product) and on CPU tensors over gloo (tests/test_multi_gpu_gloo.py).
 """
@@ -55,6 +56,30 @@ def gather_hist_partials(values, dist):
     out = torch.empty((dist.get_world_size(),) + tuple(values.shape), dtype=values.dtype, device=values.device)
     dist.all_gather(list(out.unbind(0)), values.contiguous())
     return out
+
+
+def topk_ids_to_global(ids, global_of_local):
+    """A rank's topk / bottomk ids (filo_query_device with aggr TOPK / BOTTOMK: ordinals of its table's series, -1 = empty slot) ->
+    global series ordinals through its local -> global table (a tensor on the ids' device); -1 stays -1.  Runs where the tensors are.
+    A rank whose table holds no series has only empty slots: its ids come back unchanged."""
+    import torch
+    if global_of_local.numel() == 0:
+        return ids.clone()
+    g = global_of_local.to(device=ids.device, dtype=torch.int64)
+    return torch.where(ids >= 0, g[ids.clamp(min=0)], ids)
+
+
+def gather_topk_partials(values, ids, dist):
+    """Every rank's topk / bottomk candidates ([G, T, k] f64 values and i64 global ordinals) -> two [W, G, T, k] tensors in rank order,
+    for filo_merge_topk_partials.  all_gather into views of preallocated tensors, so the same code runs on gloo and NCCL."""
+    import torch
+    # A gather, not an all-reduce: the merge selects the k best (value, ordinal) pairs of the union, which no reduction op expresses.
+    W = dist.get_world_size()
+    out_v = torch.empty((W,) + tuple(values.shape), dtype=values.dtype, device=values.device)
+    out_i = torch.empty((W,) + tuple(ids.shape), dtype=ids.dtype, device=ids.device)
+    dist.all_gather(list(out_v.unbind(0)), values.contiguous())
+    dist.all_gather(list(out_i.unbind(0)), ids.contiguous())
+    return out_v, out_i
 
 
 def max_over_ranks(x: float, dist, device) -> float:

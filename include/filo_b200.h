@@ -298,6 +298,24 @@ int32_t filo_query_hist_device(filo_ctx* ctx, const filo_table* t, int32_t range
  * is not a histogram table, or no output; FILO_ERR_UNSUPPORTED for more than 64 buckets. */
 int32_t filo_merge_hist_partials(filo_ctx* ctx, const filo_table* t, int32_t n_parts, int32_t n_windows, double quantile,
                                  const void* d_parts, void* d_out_values, void* d_out_quantile, void* cuda_stream);
+/* ReduceAggregateExec of topk / bottomk across GPUs: d_part_values / d_part_ids hold n_parts outputs of filo_query_device with
+ * aggr_op TOPK or BOTTOMK back to back, [n_parts][n_groups][n_windows][k] doubles and int64 in DEVICE memory, in rank order; every
+ * cell lists its k slots worst first, the way the query writes them.  For every (group, window) the k best non-empty candidates over
+ * all parts go to d_out_values / d_out_ids [n_groups * n_windows * k] in that same form: worst first, unused slots padded with
+ * -DBL_MAX (topk) / +DBL_MAX (bottomk) and id -1.  Better = larger value for topk, smaller for bottomk; values compare with ==
+ * (+0.0 ties -0.0), and among equal values the smaller id is better.  A slot is empty iff its id is -1 (the padding value is also a
+ * legal value); value bits pass through unchanged.  The order of the slots inside a part does not matter: the result is the k best of
+ * all non-empty slots under that rule, whatever local -> global map produced the ids.  filo_query_device never writes a NaN value with
+ * an id (NaN inputs are skipped); a NaN value with an id is skipped like an empty slot.
+ * Caller's contract: the ids are global series ordinals (map each rank's local ordinals through its local -> global table first;
+ * -1 stays -1), every part was computed with the same aggr_op, k, group numbering (n_groups) and start / step / end, and no series is
+ * in two parts.  When every part's table lists its series in increasing global ordinal (a contiguous split or the modulo shard map),
+ * the result is bit for bit the query over the union of the series, values and ids.  With another map a part keeps, among equal values
+ * at its cut, its earlier series rather than the smaller ordinals, so the merged ties may name other (equally valued) series.
+ * Enqueued on cuda_stream (NULL = ctx stream), no synchronisation.  FILO_ERR_INVALID_ARG for an operator other than TOPK / BOTTOMK,
+ * k outside [1, 32], n_parts < 1, n_groups < 1, n_windows < 1, or a NULL pointer. */
+int32_t filo_merge_topk_partials(filo_ctx* ctx, int32_t aggr_op, int32_t k, int32_t n_parts, int32_t n_groups, int32_t n_windows,
+                                 const void* d_part_values, const void* d_part_ids, void* d_out_values, void* d_out_ids, void* cuda_stream);
 
 /* Registers a region of host memory that holds chunk vectors (FiloDB's off-heap block memory, BlockManager pages) for direct
  * device access: pinned + mapped once, like the reference maps its blocks once at start-up.  filo_scan_series then lets the
