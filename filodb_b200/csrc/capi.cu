@@ -920,54 +920,16 @@ static int32_t query_device_impl(filo_ctx* ctx, const filo_table* t, int32_t fn,
   }
   const int fn_cls = fn_class_of(fn, q.cumulative, q.long_values);
   const uint64_t wrows = (uint64_t)(q.window / q.step) + 1;
-  // v3 tile kernel (scan_tile.cuh): SUM-class functions over regular series; irregular series are appended to a list that the
-  // v2 kernel processes right after, into the same output buffer.  Zero rows around a chunk let clamped windows run without
-  // bounds checks: a window spans at most window/step + 1 rows at either end; when that does not leave room for two CTAs per SM
-  // the tile kernel falls back to checked loads.
-  TileSmem TL{};
-  bool use_tile = false;
-  if (use_v2 && force != "v2" && fn_cls == CLASS_SUM && t->n_series > 0) {
-    TL = tile_layout(t->max_rec_bytes, (uint32_t)t->max_rows, (uint32_t)q.T, (uint32_t)std::min<uint64_t>(2 * wrows, 1u << 20) + 16);
-    if (((size_t)TL.total + 1024) * 2 > (size_t)228 * 1024) TL = tile_layout(t->max_rec_bytes, (uint32_t)t->max_rows, (uint32_t)q.T, 16);
-    use_tile = (size_t)TL.total + 1024 <= smem_cap;
-  }
-  // v4 SUM kernel (scan_wp.cuh): per-series rows, in front of the tile kernel; what it declines goes to the v2 kernel
-  WpSmem WL{};
-  WpBatchSmem WB{};
-  bool use_wp = false, use_wp_batch = false;
-  if (use_tile && force != "v3" && wrows <= 4096 && t->max_chunks > 0) {
-    // O in V's place (more warps per SM) when every series is summed in one pass of <= 64 blocks
-    const bool alias = wp_max_items((uint32_t)t->max_chunks, (uint32_t)q.T, (uint32_t)wrows) <= 64;
-    WL = wp_layout(t->max_rec_bytes, (uint32_t)t->max_rows, (uint32_t)t->max_chunks, (uint32_t)q.T, (uint32_t)wrows, alias);
-    WL.warps = (uint32_t)std::min<size_t>(smem_cap / WL.per_warp, alias ? WP_MAX_WARPS_ALIAS : WP_MAX_WARPS);
-    // two record buffers per warp (the records of the next two series in flight) when 16 warps of them fit
-    const WpSmem WL2 = wp_layout(t->max_rec_bytes, (uint32_t)t->max_rows, (uint32_t)t->max_chunks, (uint32_t)q.T, (uint32_t)wrows, alias, true);
-    if (smem_cap / WL2.per_warp >= (size_t)WP_MAX_WARPS) {
-      WL = WL2; WL.warps = WP_MAX_WARPS;
-      // that layout's record bytes as one CTA-wide stream: batches of consecutive records, a producer warp parses their headers.  Its
-      // layout adds the raw tail area behind the result row (no bytes for C2: the row and the area fit in V's region); where that does
-      // not fit, the table stays on scan_wp_sum_kernel with two record buffers per warp
-      WB = wp_batch_layout(t->max_rec_bytes, (uint32_t)t->max_rows, (uint32_t)t->max_chunks, (uint32_t)q.T, (uint32_t)wrows, alias);
-      use_wp_batch = WB.total <= smem_cap;
-      // the batch kernel's window blocks write finished windows over O right after the pass's reads of V: with O on V every plan must be
-      // one pass of at most 64 blocks
-      if (use_wp_batch && WB.W.alias && wp_max_items((uint32_t)t->max_chunks, (uint32_t)q.T, (uint32_t)wrows) > 64)
-        return fail(ctx, FILO_ERR_UNSUPPORTED, "scan_wp_batch_kernel: O on V with plans of more than one pass");
-    }
-    use_wp = WL.warps >= 4;
-  }
-  // v4 counter-class kernel (scan_wp_ctr.cuh): per-series rows, or fused partial rows of up to TILE_AGG_ACC * TILE_THREADS windows;
+  // the per-series kernel in front of v2 (scan_path, scan_wp_layout.h): the v4 SUM kernels, the tile kernel or the v4 counter kernel;
   // what it declines goes to the v2 kernel
-  WpCtrSmem WC{};
-  bool use_wp_ctr = false;
-  if (use_v2 && force != "v2" && force != "v3" && fn_cls == CLASS_COUNTER && t->n_series > 0 && t->max_chunks > 0 &&
-      (!fused || q.T <= TILE_AGG_ACC * TILE_THREADS) && wp_ctr_tile_footprint_ok(t->max_rec_bytes, (uint32_t)t->max_rows, (uint32_t)q.T, smem_cap)) {
-    WC = wp_ctr_layout(t->max_rec_bytes, (uint32_t)t->max_rows, (uint32_t)t->max_chunks, (uint32_t)q.T, fused, t->any_nonconst_ts, moments);
-    // the irregular-timestamp instantiation is built for <= 16 warps
-    const size_t w = std::min<size_t>((smem_cap - sizeof(TileCtrTab) * (TILE_CTR_TABMAX + 1) - 64) / WC.per_warp, WC.tsr != 0 ? 16 : WP_CTR_MAX_WARPS);
-    WC.warps = (uint32_t)w; WC.tab = (uint32_t)(WC.per_warp * w);
-    use_wp_ctr = w >= 4;
-  }
+  ScanPathIn pin{};
+  pin.max_rec_bytes = t->max_rec_bytes; pin.max_rows = (uint32_t)t->max_rows; pin.max_chunks = (uint32_t)t->max_chunks; pin.T = (uint32_t)q.T;
+  pin.wrows = wrows; pin.fn_cls = fn_cls; pin.fused = fused; pin.moments = moments; pin.irr = t->any_nonconst_ts; pin.v2 = use_v2;
+  pin.force = force == "v2" ? 2 : force == "v3" ? 3 : 0; pin.smem_cap = smem_cap; pin.n_series = t->n_series; pin.sm_count = ctx->sm_count;
+  const ScanPath SP = scan_path(pin);
+  if (SP.refused) return fail(ctx, FILO_ERR_UNSUPPORTED, "scan_wp_batch_kernel: O on V with plans of more than one pass");
+  const TileSmem& TL = SP.TL; const WpSmem& WL = SP.WL; const WpBatchSmem& WB = SP.WB; const WpCtrSmem& WC = SP.WC;
+  const bool use_tile = SP.tile, use_wp_ctr = SP.wp_ctr;
   auto run_per_series = [&](double* outp) -> int32_t {
     if (use_tile || use_wp_ctr) {
       int64_t* d_list = nullptr; unsigned long long* d_cnt = nullptr;
@@ -976,19 +938,14 @@ static int32_t query_device_impl(filo_ctx* ctx, const filo_table* t, int32_t fn,
       CUDA_TRY(ctx, cudaMemsetAsync(d_cnt, 0, 16, s));
       ScanLaunch LT = L;
       static const bool dbg = std::getenv("FILO_DEBUG_SYNC") != nullptr;
-      if (use_wp_batch) {
-        LT.grid = (int)std::max<int64_t>(1, std::min<int64_t>((t->n_series + WB.B - 1) / WB.B, (int64_t)ctx->sm_count));
+      LT.grid = SP.grid;
+      if (SP.kernel == SCAN_PATH_WP_BATCH) {
         CUDA_TRY(ctx, launch_scan_wp_batch(LT, outp, WB, d_list, d_cnt));
-      } else if (use_wp) {
-        LT.grid = (int)std::max<int64_t>(1, std::min<int64_t>((t->n_series + WL.warps - 1) / WL.warps, (int64_t)ctx->sm_count));
+      } else if (SP.kernel == SCAN_PATH_WP_SUM) {
         CUDA_TRY(ctx, launch_scan_wp(LT, outp, WL, d_list, d_cnt));
-      } else if (use_wp_ctr) {
-        LT.grid = (int)std::max<int64_t>(1, std::min<int64_t>((t->n_series + WC.warps - 1) / WC.warps, (int64_t)ctx->sm_count));
+      } else if (SP.kernel == SCAN_PATH_WP_CTR) {
         CUDA_TRY(ctx, launch_scan_wp_ctr(LT, outp, WC, d_list, d_cnt));
       } else {
-        const int ctas_per_sm = ((size_t)TL.total + 1024) * 2 <= (size_t)228 * 1024 ? 2 : 1;
-        const int64_t n_tiles = (t->n_series + TILE_NS - 1) / TILE_NS;
-        LT.grid = (int)std::max<int64_t>(1, std::min<int64_t>(n_tiles, (int64_t)ctx->sm_count * ctas_per_sm));
         if (dbg) { fprintf(stderr, "[filo] tile kernel fn=%d T=%d grid=%d smem=%u pitch=%u\n", fn, q.T, LT.grid, TL.total, TL.vals_pitch); fflush(stderr); }
         CUDA_TRY(ctx, launch_scan_tile(LT, outp, TL, d_list, d_cnt));
       }
@@ -1029,8 +986,7 @@ static int32_t query_device_impl(filo_ctx* ctx, const filo_table* t, int32_t fn,
         LT.grid = (int)std::max<int64_t>(1, std::min<int64_t>((t->n_items + WC.warps - 1) / WC.warps, (int64_t)ctx->sm_count));
         CUDA_TRY(ctx, launch_scan_wp_ctr_agg(LT, WC, order, t->d_item_begin, t->n_items, scan_op, pval, pcnt, d_list, d_cnt, moments));
       } else {
-        const int ctas_per_sm = ((size_t)TL.total + 1024) * 2 <= (size_t)228 * 1024 ? 2 : 1;
-        LT.grid = (int)std::max<int64_t>(1, std::min<int64_t>(t->n_items, (int64_t)ctx->sm_count * ctas_per_sm));
+        LT.grid = (int)std::max<int64_t>(1, std::min<int64_t>(t->n_items, (int64_t)ctx->sm_count * SP.tile_ctas_per_sm));
         CUDA_TRY(ctx, launch_scan_tile_agg(LT, TL, order, t->d_item_begin, t->n_items, scan_op, pval, pcnt, d_list, d_cnt, moments));
       }
       ScanLaunch LF = L; LF.list = d_list; LF.list_count = d_cnt;

@@ -192,4 +192,80 @@ FILO_HD inline bool wp_ctr_tile_footprint_ok(uint32_t max_rec_bytes, uint32_t ma
   return (uint64_t)(tile_layout(max_rec_bytes, max_rows, T, 0).total + ctr) + 1024 <= cap;
 }
 
+// ---- the per-series kernel a query runs in front of the v2 kernel (filo_query); the v2 kernel takes what that kernel declines
+enum { SCAN_PATH_V2 = 0, SCAN_PATH_TILE = 1, SCAN_PATH_WP_SUM = 2, SCAN_PATH_WP_BATCH = 3, SCAN_PATH_WP_CTR = 4 };
+struct ScanPathIn {
+  uint32_t max_rec_bytes, max_rows, max_chunks, T;   // the table's largest record, rows and chunks per series; windows
+  uint64_t wrows;                      // window / step + 1
+  int fn_cls;                          // fn_class_of
+  bool fused, moments;                 // an across-series aggregate folded in the scan kernels; stddev / stdvar
+  bool irr;                            // the table has series whose timestamps are not const-DDV
+  bool v2;                             // the v2 kernel takes the table (its per-warp working set fits)
+  int force;                           // FILO_KERNEL: 2 keeps every class on v2, 3 keeps the SUM class on the tile kernel; 0 otherwise
+  uint64_t smem_cap;                   // shared memory one CTA may opt into
+  int64_t n_series;
+  int sm_count;
+};
+struct ScanPath {
+  int kernel;                          // SCAN_PATH_*: the per-series kernel
+  bool tile, wp, wp_batch, wp_ctr;     // tile: the tile layout fits (it also serves fused SUM-class aggregates); the v4 kernels in front of it
+  bool refused;                        // the batch kernel with O on V and plans of more than one pass: the query is refused
+  int tile_ctas_per_sm;
+  int grid;                            // CTAs of the per-series kernel (persistent: at most one per SM for the v4 kernels)
+  TileSmem TL; WpSmem WL; WpBatchSmem WB; WpCtrSmem WC;
+};
+FILO_HD inline ScanPath scan_path(const ScanPathIn& in) {
+  ScanPath P{};
+  P.kernel = SCAN_PATH_V2;
+  const uint32_t T = in.T, wrows = (uint32_t)in.wrows;
+  // v3 tile kernel (scan_tile.cuh): SUM-class functions over regular series.  Zero rows around a chunk let clamped windows run without
+  // bounds checks: a window spans at most window/step + 1 rows at either end; when that does not leave room for two CTAs per SM the
+  // tile kernel falls back to checked loads.
+  if (in.v2 && in.force != 2 && in.fn_cls == CLASS_SUM && in.n_series > 0) {
+    P.TL = tile_layout(in.max_rec_bytes, in.max_rows, T, (uint32_t)(2 * in.wrows < (1u << 20) ? 2 * in.wrows : (1u << 20)) + 16);
+    if (((uint64_t)P.TL.total + 1024) * 2 > (uint64_t)228 * 1024) P.TL = tile_layout(in.max_rec_bytes, in.max_rows, T, 16);
+    P.tile = (uint64_t)P.TL.total + 1024 <= in.smem_cap;
+  }
+  P.tile_ctas_per_sm = ((uint64_t)P.TL.total + 1024) * 2 <= (uint64_t)228 * 1024 ? 2 : 1;
+  // v4 SUM kernel (scan_wp.cuh): per-series rows, in front of the tile kernel
+  if (P.tile && in.force != 3 && in.wrows <= 4096 && in.max_chunks > 0) {
+    // O in V's place (more warps per SM) when every series is summed in one pass of <= 64 blocks
+    const bool alias = wp_max_items(in.max_chunks, T, wrows) <= 64;
+    P.WL = wp_layout(in.max_rec_bytes, in.max_rows, in.max_chunks, T, wrows, alias);
+    { const uint64_t w = in.smem_cap / P.WL.per_warp, wmax = alias ? WP_MAX_WARPS_ALIAS : WP_MAX_WARPS; P.WL.warps = (uint32_t)(w < wmax ? w : wmax); }
+    // two record buffers per warp (the records of the next two series in flight) when 16 warps of them fit
+    const WpSmem WL2 = wp_layout(in.max_rec_bytes, in.max_rows, in.max_chunks, T, wrows, alias, true);
+    if (in.smem_cap / WL2.per_warp >= (uint64_t)WP_MAX_WARPS) {
+      P.WL = WL2; P.WL.warps = WP_MAX_WARPS;
+      // that layout's record bytes as one CTA-wide stream: batches of consecutive records, a producer warp parses their headers.  Its
+      // layout adds the raw tail area behind the result row (no bytes for C2: the row and the area fit in V's region); where that does
+      // not fit, the table stays on scan_wp_sum_kernel with two record buffers per warp
+      P.WB = wp_batch_layout(in.max_rec_bytes, in.max_rows, in.max_chunks, T, wrows, alias);
+      P.wp_batch = P.WB.total <= in.smem_cap;
+      // the batch kernel's window blocks write finished windows over O right after the pass's reads of V: with O on V every plan must be
+      // one pass of at most 64 blocks
+      if (P.wp_batch && P.WB.W.alias && wp_max_items(in.max_chunks, T, wrows) > 64) P.refused = true;
+    }
+    P.wp = P.WL.warps >= 4;
+  }
+  // v4 counter-class kernel (scan_wp_ctr.cuh): per-series rows, or fused partial rows of up to TILE_AGG_ACC * TILE_THREADS windows
+  if (in.v2 && in.force != 2 && in.force != 3 && in.fn_cls == CLASS_COUNTER && in.n_series > 0 && in.max_chunks > 0 &&
+      (!in.fused || T <= (uint32_t)(TILE_AGG_ACC * TILE_THREADS)) && wp_ctr_tile_footprint_ok(in.max_rec_bytes, in.max_rows, T, in.smem_cap)) {
+    P.WC = wp_ctr_layout(in.max_rec_bytes, in.max_rows, in.max_chunks, T, in.fused, in.irr, in.moments);
+    // the irregular-timestamp instantiation is built for <= 16 warps
+    const uint64_t w = (in.smem_cap - sizeof(TileCtrTab) * (TILE_CTR_TABMAX + 1) - 64) / P.WC.per_warp, wmax = P.WC.tsr != 0 ? 16 : WP_CTR_MAX_WARPS;
+    P.WC.warps = (uint32_t)(w < wmax ? w : wmax); P.WC.tab = (uint32_t)(P.WC.per_warp * P.WC.warps);
+    P.wp_ctr = P.WC.warps >= 4;
+  }
+  // the per-series kernel and its grid
+  const int64_t n = in.n_series, sms = in.sm_count;
+  int64_t g = 1;
+  if (P.wp_batch)    { P.kernel = SCAN_PATH_WP_BATCH; g = (n + P.WB.B - 1) / P.WB.B; if (g > sms) g = sms; }
+  else if (P.wp)     { P.kernel = SCAN_PATH_WP_SUM;   g = (n + P.WL.warps - 1) / P.WL.warps; if (g > sms) g = sms; }
+  else if (P.wp_ctr) { P.kernel = SCAN_PATH_WP_CTR;   g = (n + P.WC.warps - 1) / P.WC.warps; if (g > sms) g = sms; }
+  else if (P.tile)   { P.kernel = SCAN_PATH_TILE;     g = (n + TILE_NS - 1) / TILE_NS; if (g > sms * P.tile_ctas_per_sm) g = sms * P.tile_ctas_per_sm; }
+  P.grid = (int)(g > 1 ? g : 1);
+  return P;
+}
+
 } // namespace filo
