@@ -12,6 +12,7 @@ namespace filo { alignas(128) uint8_t smem[232448]; }          // `extern __shar
 #include "../../filodb_b200/csrc/scan_kernels.cu"          // every scan kernel (the launchers are compiled out under FILO_CUSIM)
 #endif
 #include "../../oracle/filo_query.hpp"
+#include <cassert>
 #include <memory>
 #include <random>
 #include <string>
@@ -23,11 +24,13 @@ static long g_wp_declined = 0, g_wp_series = 0;
 static int g_long_col = 0;          // 1: Long value column through LongBinaryVector.optimize (DDV / const DDV), 2: raw 64-bit longs
 static int g_jitter_ms = 0; static bool g_integral = false;      // irregular scrapes (DDV timestamps) / integral values (DoubleVector.optimize -> DDV longs)
 static bool g_signed_zero = false;  // gauge values +0.0 / -0.0 in runs of 12 rows: min / max meet equal zeros of both signs
+static std::string g_chunk_enc;     // when set: chunk c's values XOR ('x') or raw f64 ('r'), in place of xor_enc
 // chunks of the given rows (nan_ppm: a stale marker at a chunk end) and the arena record, from timestamps and values
 static void build_series_from(SeriesData& S, std::mt19937_64& rng, const std::vector<int64_t>& ts, const std::vector<double>& v, const std::vector<int>& chunk_rows,
                               int kind /*0 gauge 1 counter*/, bool xor_enc, int nan_ppm) {
   int r0 = 0;
   for (int n : chunk_rows) {
+    if (!g_chunk_enc.empty()) { assert(g_chunk_enc.size() == chunk_rows.size()); xor_enc = g_chunk_enc[S.chunks.size()] == 'x'; }
     auto c = std::make_unique<Chunk>();
     std::vector<double> cv(v.begin() + r0, v.begin() + r0 + n);
     if (nan_ppm && (int)(rng() % 1000000) < nan_ppm) cv[(size_t)n - 1] = std::nan("");          // stale marker at the chunk end
