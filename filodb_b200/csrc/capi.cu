@@ -925,7 +925,7 @@ static int32_t query_device_impl(filo_ctx* ctx, const filo_table* t, int32_t fn,
   ScanPathIn pin{};
   pin.max_rec_bytes = t->max_rec_bytes; pin.max_rows = (uint32_t)t->max_rows; pin.max_chunks = (uint32_t)t->max_chunks; pin.T = (uint32_t)q.T;
   pin.wrows = wrows; pin.fn_cls = fn_cls; pin.fused = fused; pin.moments = moments; pin.irr = t->any_nonconst_ts; pin.v2 = use_v2;
-  pin.force = force == "v2" ? 2 : force == "v3" ? 3 : 0; pin.smem_cap = smem_cap; pin.n_series = t->n_series; pin.sm_count = ctx->sm_count;
+  pin.force = force == "v2" ? 2 : force == "v3" ? 3 : 0; pin.smem_cap = smem_cap; pin.n_series = t->n_series; pin.n_items = t->n_items; pin.sm_count = ctx->sm_count;
   const ScanPath SP = scan_path(pin);
   if (SP.refused) return fail(ctx, FILO_ERR_UNSUPPORTED, "scan_wp_batch_kernel: O on V with plans of more than one pass");
   const TileSmem& TL = SP.TL; const WpSmem& WL = SP.WL; const WpBatchSmem& WB = SP.WB; const WpCtrSmem& WC = SP.WC;
@@ -975,18 +975,17 @@ static int32_t query_device_impl(filo_ctx* ctx, const filo_table* t, int32_t fn,
     CUDA_TRY(ctx, tmp.alloc((void**)&pval, (size_t)t->n_items * q.T * 8 * (moments ? 2 : 1)));      // moments: [2][n_items][T]
     CUDA_TRY(ctx, tmp.alloc((void**)&pcnt, (size_t)t->n_items * q.T * 4));
     const int32_t* order = t->grouped ? t->d_order : nullptr;
-    if ((use_tile && q.T <= TILE_AGG_ACC * TILE_THREADS) || use_wp_ctr) {
+    if (SP.fused_kernel != SCAN_PATH_V2) {
       // the tile / v4 counter kernel folds every item into one partial row; items with a series it declines go through the v2 kernel
       int64_t* d_list = nullptr; unsigned long long* d_cnt = nullptr;
       CUDA_TRY(ctx, tmp.alloc((void**)&d_list, (size_t)t->n_items * 8));
       CUDA_TRY(ctx, tmp.alloc((void**)&d_cnt, 16));
       CUDA_TRY(ctx, cudaMemsetAsync(d_cnt, 0, 16, s));
       ScanLaunch LT = L;
-      if (use_wp_ctr) {
-        LT.grid = (int)std::max<int64_t>(1, std::min<int64_t>((t->n_items + WC.warps - 1) / WC.warps, (int64_t)ctx->sm_count));
+      LT.grid = SP.fused_grid;
+      if (SP.fused_kernel == SCAN_PATH_WP_CTR) {
         CUDA_TRY(ctx, launch_scan_wp_ctr_agg(LT, WC, order, t->d_item_begin, t->n_items, scan_op, pval, pcnt, d_list, d_cnt, moments));
       } else {
-        LT.grid = (int)std::max<int64_t>(1, std::min<int64_t>(t->n_items, (int64_t)ctx->sm_count * SP.tile_ctas_per_sm));
         CUDA_TRY(ctx, launch_scan_tile_agg(LT, TL, order, t->d_item_begin, t->n_items, scan_op, pval, pcnt, d_list, d_cnt, moments));
       }
       ScanLaunch LF = L; LF.list = d_list; LF.list_count = d_cnt;

@@ -204,6 +204,7 @@ struct ScanPathIn {
   int force;                           // FILO_KERNEL: 2 keeps every class on v2, 3 keeps the SUM class on the tile kernel; 0 otherwise
   uint64_t smem_cap;                   // shared memory one CTA may opt into
   int64_t n_series;
+  int64_t n_items;                     // work items of the table's grouping (build_groups_new): the fused kernels' work
   int sm_count;
 };
 struct ScanPath {
@@ -212,6 +213,9 @@ struct ScanPath {
   bool refused;                        // the batch kernel with O on V and plans of more than one pass: the query is refused
   int tile_ctas_per_sm;
   int grid;                            // CTAs of the per-series kernel (persistent: at most one per SM for the v4 kernels)
+  int fused_kernel;                    // fused aggregates: SCAN_PATH_WP_CTR or SCAN_PATH_TILE in front of the v2 aggregate kernel, or
+                                       // SCAN_PATH_V2 (the v2 / v1 aggregate kernel alone)
+  int fused_grid;                      // CTAs of the fused ctr / tile kernel (items are strided over warps / CTAs); 0 for SCAN_PATH_V2
   TileSmem TL; WpSmem WL; WpBatchSmem WB; WpCtrSmem WC;
 };
 FILO_HD inline ScanPath scan_path(const ScanPathIn& in) {
@@ -265,6 +269,15 @@ FILO_HD inline ScanPath scan_path(const ScanPathIn& in) {
   else if (P.wp_ctr) { P.kernel = SCAN_PATH_WP_CTR;   g = (n + P.WC.warps - 1) / P.WC.warps; if (g > sms) g = sms; }
   else if (P.tile)   { P.kernel = SCAN_PATH_TILE;     g = (n + TILE_NS - 1) / TILE_NS; if (g > sms * P.tile_ctas_per_sm) g = sms * P.tile_ctas_per_sm; }
   P.grid = (int)(g > 1 ? g : 1);
+  // the fused kernel and its grid: the counter kernel folds warp gw's items gw, gw + warps * grid, ..; the tile kernel CTA c's items
+  // c, c + grid, ..; the tile kernel's accumulators hold TILE_AGG_ACC * TILE_THREADS windows
+  const int64_t ni = in.n_items;
+  P.fused_kernel = SCAN_PATH_V2; P.fused_grid = 0;
+  if (P.wp_ctr) {
+    P.fused_kernel = SCAN_PATH_WP_CTR; g = (ni + P.WC.warps - 1) / P.WC.warps; if (g > sms) g = sms; P.fused_grid = (int)(g > 1 ? g : 1);
+  } else if (P.tile && T <= (uint32_t)(TILE_AGG_ACC * TILE_THREADS)) {
+    P.fused_kernel = SCAN_PATH_TILE; g = ni; if (g > sms * P.tile_ctas_per_sm) g = sms * P.tile_ctas_per_sm; P.fused_grid = (int)(g > 1 ? g : 1);
+  }
   return P;
 }
 

@@ -1,8 +1,8 @@
 // The per-series kernel filo_query runs for one table shape (scan_path, scan_wp_layout.h), with its layout, its grid and how deep
 // into a persistent grid the table's series reach: series per warp and the last buffer round every warp gets to.  Test
-// infrastructure: built with g++ and run by tests/test_scan_path.py and tests/test_gpu_steady_state.py.
+// infrastructure: built with g++ and run by tests/test_scan_path.py, tests/test_gpu_steady_state.py and tests/test_gpu_fused_steady_state.py.
 //   scan_path rec=<max_rec_bytes> rows=<max_rows> chunks=<max_chunks> T=<windows> wrows=<window / step + 1> n=<series>
-//             [cls=sum|counter|minmax|point] [fused=0|1] [moments=0|1] [irr=0|1] [v2=0|1] [smem=<cap bytes>] [sms=<SMs>]
+//             [cls=sum|counter|minmax|point] [fused=0|1 items=<work items>] [moments=0|1] [irr=0|1] [v2=0|1] [smem=<cap bytes>] [sms=<SMs>]
 // v2=1 (the default) says the v2 kernel's per-warp working set fits, which filo_query checks before it asks scan_path.
 // Prints one key=value per line:
 //   kernel      batch | sum | tile | ctr | v2 (batch: scan_wp_batch_kernel, sum: scan_wp_sum_kernel, ctr: scan_wp_ctr_kernel)
@@ -13,6 +13,11 @@
 //   grid, smem  CTAs and dynamic shared memory per CTA
 //   series_per_warp  the fewest series any warp takes (tile: the fewest tiles any CTA takes)
 //   rounds      the last buffer round u = k / rec_bufs every warp reaches (k: the warp's series index from 0); -1 below one series
+// and with fused=1, the fused aggregate path over `items` work items:
+//   fused_kernel    ctr | tile | v2 (ctr: scan_wp_ctr_kernel<AGG>, tile: scan_tile_kernel<AGG>, each with scan_agg_kernel_v2 behind it
+//                   for the items it declines; v2: the v2 / v1 aggregate kernel alone)
+//   fused_grid      CTAs of the ctr / tile kernel (0 for v2)
+//   items_per_warp  the fewest items any warp (ctr) or CTA (tile) takes; -1 for v2
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -35,6 +40,7 @@ int main(int argc, char** argv) {
     else if (k == "T") in.T = (uint32_t)x;
     else if (k == "wrows") in.wrows = (uint64_t)x;
     else if (k == "n") in.n_series = x;
+    else if (k == "items") in.n_items = x;
     else if (k == "cls") {
       if (v == "sum") in.fn_cls = CLASS_SUM; else if (v == "counter") in.fn_cls = CLASS_COUNTER;
       else if (v == "minmax") in.fn_cls = CLASS_MINMAX; else if (v == "point") in.fn_cls = CLASS_POINT;
@@ -84,5 +90,12 @@ int main(int argc, char** argv) {
   std::printf("kernel=%s\nalias=%lld\nwarps=%lld\nrec_bufs=%lld\nB=%lld\ngrid=%lld\nsmem=%lld\nseries_per_warp=%lld\nrounds=%lld\n", name,
               (long long)alias, (long long)warps, (long long)bufs, (long long)B, (long long)grid, (long long)smem, (long long)fewest,
               (long long)rounds);
+  if (in.fused) {
+    // ctr: warp gw takes items gw + k * (grid * warps); tile: CTA c takes items c + k * grid
+    const int64_t ni = in.n_items, fg = P.fused_grid;
+    const char* fname = P.fused_kernel == SCAN_PATH_WP_CTR ? "ctr" : P.fused_kernel == SCAN_PATH_TILE ? "tile" : "v2";
+    const int64_t per = P.fused_kernel == SCAN_PATH_WP_CTR ? ni / (fg * (int64_t)P.WC.warps) : P.fused_kernel == SCAN_PATH_TILE ? ni / fg : -1;
+    std::printf("fused_kernel=%s\nfused_grid=%lld\nitems_per_warp=%lld\n", fname, (long long)fg, (long long)per);
+  }
   return 0;
 }
